@@ -3,6 +3,7 @@
 
   python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
   python bench.py --impl reference --steps K --warmup W    # the reference algorithm on the host CPU (oracle port)
+  python bench.py --steps K --dump-outputs DIR              # also write the last timed step's outputs as DIR/<name>.npy
 
 One step = one loop body of generate_samples_from_batch (reference model_v2w.py:130-149): sampler glue +
 cond forward + uncond forward of the 28-block 7B DiT over the 121-frame / 704x1280 latent [16,16,88,160]
@@ -44,11 +45,12 @@ def measured_peaks():
         d = json.load(open(p))
         return {"tflops_burst": d["bf16_tflops"], "tflops_sustained": d["bf16_tflops_sustained"], "hbm_gbs": d["hbm_gbs"],
                 "source": "measured"}
-    return {"tflops_burst": 1590.0, "tflops_sustained": 1400.0, "hbm_gbs": 6650.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (dense BF16, HBM3), for a card allowed 700 W; a power-capped card reaches less
+    return {"tflops_burst": 989.0, "tflops_sustained": 989.0, "hbm_gbs": 3350.0, "source": "datasheet"}
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -193,7 +195,7 @@ def path_r_cpu_frames_per_s(n_frames: int = 4):
     return n_frames / dt, dt, 1
 
 
-def bench_path_r(torch, dev, peaks, steps: int, warmup: int, cpu_baseline: bool):
+def bench_path_r(torch, dev, peaks, steps: int, warmup: int, cpu_baseline: bool, last: dict | None = None):
     import numpy as np
 
     from gen3c_b200 import warp
@@ -227,6 +229,8 @@ def bench_path_r(torch, dev, peaks, steps: int, warmup: int, cpu_baseline: bool)
         pix, msk = warp.render_cache(c.input_points[:, :, :, 0], c.input_image[:, :, :, 0], None,
                                      w2cs_h.to(dev, non_blocking=True), Ks_h.to(dev, non_blocking=True))
         cov_h.copy_(msk.mean(dim=(0, 2, 3, 4, 5)), non_blocking=True)
+        if last is not None:
+            last["pixels"], last["masks"] = pix, msk
         return pix
 
     def timed(fn, n):
@@ -241,7 +245,7 @@ def bench_path_r(torch, dev, peaks, steps: int, warmup: int, cpu_baseline: bool)
 
     for i in range(max(3, warmup)):
         resident(i)
-    n = max(steps, 10)
+    n = steps
     ms = timed(resident, n)
     e2e(0)
     ms_e2e = timed(e2e, n)
@@ -259,7 +263,6 @@ def bench_path_r(torch, dev, peaks, steps: int, warmup: int, cpu_baseline: bool)
                            "stay on the GPU as in the reference (cache_3d.py:236), per-frame coverage is read back"},
            "roofline": {"bound": "hbm", "kernel": "k_splat_points (+ k_project_max, k_normalise)", "achieved": gbs,
                         "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": gbs / peaks["hbm_gbs"],
-                        "traffic": ncu_traffic_bytes("r02_splat_ncu_summary.txt"),
                         "algorithmic_bytes_per_render": px * R_BYTES_PER_PX, "peak_source": peaks["source"]}}
     if cpu_baseline:
         fps, dt, thr = path_r_cpu_frames_per_s(4)
@@ -519,6 +522,8 @@ def run_ours(args):
     step_e2e(0)
     ms_e2e = timed(step_e2e, args.steps)
     clk = clocks.finish()
+    # out_host holds x_(t-1) of the last timed step (step args.steps - 1), as the caller of the public API receives it
+    dump = {"x_next": out_host.float().numpy()} if args.dump_outputs else None
     if rank != 0:
         if world > 1:
             net._teardown_barrier()
@@ -549,12 +554,9 @@ def run_ours(args):
                    "parallelism": par_name, "l2": "inputs larger than L2 (14.5 GB weights, 0.9 GB residual stream)"},
         "e2e": {"value": 1e3 / ms_e2e, "unit": "steps/s", "h2d_bytes_per_step": h2d_bytes, "d2h_bytes_per_step": d2h_bytes},
         "gpu_launches": launches_per_step * args.steps,
-        "roofline": {"bound": "tensor", "kernel": "k_attn_fwd1t (self-attention)", "achieved": achieved, "peak": peak,
+        "roofline": {"bound": "tensor", "kernel": "k_attn_fwd (self-attention)", "achieved": achieved, "peak": peak,
                      "unit": "TFLOP/s", "frac": achieved / peak,
-                     # DRAM bytes of one launch from the committed ncu --set full capture of this kernel at the cp = 1
-                     # shape; not meaningful for the sharded shapes, hence null there
-                     "traffic": ncu_traffic_bytes("r02_attn_ncu_summary.txt", "r01_attn_ncu_summary.txt") if cp_size == 1 else None,
-                     "peak_source": peaks["source"] + " (sustained)",
+                     "peak_source": peaks["source"] + (" (sustained)" if peaks["source"] == "measured" else ""),
                      "step_tflops": FLOP_PER_STEP * sps / 1e12 / world, "step_frac": FLOP_PER_STEP * sps / 1e12 / world / peak},
         "kernel_breakdown": breakdown,
         "clocks": clk,
@@ -585,38 +587,34 @@ def run_ours(args):
     if world == 1 and not args.no_path_r:
         del devt
         torch.cuda.empty_cache()
+        last_r = {} if dump is not None else None
         try:
-            line["path_r"] = bench_path_r(torch, dev, peaks, args.steps, args.warmup, not args.no_cpu_baseline)
+            line["path_r"] = bench_path_r(torch, dev, peaks, args.steps, args.warmup, not args.no_cpu_baseline, last_r)
         except Exception as ex:  # noqa: BLE001 - the second leg must never cost the headline line
             line["path_r"] = {"error": repr(ex)[:300]}
+        if last_r:
+            # the render is 1.7 GB: a fixed, seeded sample of 2^20 elements of each output
+            for name, t in (("path_r_pixels", last_r["pixels"]), ("path_r_masks", last_r["masks"])):
+                flat = t.reshape(-1)
+                idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(2024))[:1 << 20].sort().values
+                dump[name] = flat[idx.to(flat.device)].float().cpu().numpy()
+    if dump is not None:
+        write_dump(args.dump_outputs, dump)
     print(json.dumps(line), flush=True)
     if world > 1:
         net._teardown_barrier()
         dist.destroy_process_group()
 
 
-def ncu_traffic_bytes(*names):
-    """DRAM bytes (read + write) of one launch of the named kernel, from the first committed `ncu --set full` summary found
-    under profiles/ (written by tools/ncu_summary.py from the capture of the same shape); None when absent.  Static
-    evidence: bench.py cannot read DRAM counters itself (a number printed under a profiler is never a bench value)."""
-    scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9, "Tbyte": 1e12}
-    for name in names:
-        path = os.path.join(ROOT, "profiles", name)
-        tot, seen = 0.0, 0
-        try:
-            for ln in open(path):
-                if ln.startswith("--") and seen >= 2:
-                    break
-                for key in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                    if ln.startswith(key):
-                        unit = ln[ln.index("[") + 1:ln.index("]")]
-                        tot += float(ln.split("=")[1]) * scale[unit]
-                        seen += 1
-        except (OSError, ValueError, KeyError):
-            continue
-        if seen >= 2:
-            return tot
-    return None
+def write_dump(out_dir: str, arrays: dict):
+    """--dump-outputs: every array as out_dir/<name>.npy in float32 (64 MB in all at most)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    total = sum(a.size * 4 for a in arrays.values())
+    assert total <= 64 << 20, f"dump of {total} bytes exceeds 64 MB"
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a, dtype=np.float32))
 
 
 def main():
@@ -628,6 +626,9 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the attention A/B and the torch-kernel reference-graph arm")
     ap.add_argument("--no-path-r", action="store_true", help="skip the 3D-cache render leg")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (float32): "
+                         "x_next = x_(t-1) of the denoise step, and seeded samples of the Path R render")
     ap.add_argument("--parallelism", default="auto", choices=["auto", "cp", "cfgxcp"],
                     help="N > 1: cfgxcp (default) = cond / uncond forward on two halves of the ranks x context parallel "
                          "inside each half; cp = context parallel over all ranks (the reference's layout)")

@@ -1,4 +1,4 @@
-"""gen3c_b200 — Blackwell-native (sm_100a) engine for GEN3C's two hot paths.
+"""gen3c_b200 — Hopper-native (sm_90a, H100) engine for GEN3C's two hot paths.
 
 Path R (3D-cache render): ``gen3c_b200.warp`` / ``gen3c_b200.cache_3d``
 Path D (7B DiT denoise step): ``gen3c_b200.dit`` / ``gen3c_b200.sampler`` / ``gen3c_b200.ops``

@@ -1,0 +1,331 @@
+// Path D — non-causal multi-head attention forward, head_dim 128, on the Hopper tensor cores (wgmma).
+//   O = softmax(Q K^T * scale) V        (reference: cosmos_predict1/diffusion/module/attention.py
+//   :282-297 `cal_attn` -> transformer_engine DotProductAttention(sbhd, no_mask, dropout 0);
+//   self-attention Lq = Lk = 56 320, cross-attention Lk = 512; SURVEY.md §8a row D9)
+//
+// Layouts (all bf16, produced by the projection GEMMs of gemm_wgmma.cu):
+//   Q  [Lq, heads*128]  token-major          K [Lk, heads*128] token-major
+//   Vt [chunks][heads*128][chunk_len]        (V transposed, keys contiguous -> K-major B operand;
+//                                             `chunks` = context-parallel ranks after the KV
+//                                             all-gather, 1 otherwise)
+//   O  [Lq, heads*128]
+//
+// One CTA = 128 query rows of one head, 384 threads (three warpgroups):
+//   warpgroup 0     TMA producer: Q once, then K_j / V^T_j through a ring of ATT_STAGES 64 KB stages (separate
+//                   barriers for K and V, so S = Q K^T of a step starts before its V has landed)
+//   warpgroups 1-2  consumers, 64 query rows each:  S = Q K_j^T (wgmma, A and B from shared memory) -> online
+//                   softmax in registers (exact row max per 128-key tile, rescale of O) -> P converted in
+//                   place to the bf16 A fragments of O += P V_j (wgmma with A from registers).
+// The two consumer warpgroups run the same step independently, so the softmax of one overlaps the MMAs of the other.
+#include <cmath>
+#include <cstdlib>
+
+#include "kernels.h"
+
+namespace g3c {
+
+constexpr int ATT_THREADS = 384;
+constexpr int ATT_TILE = 128;              // query rows per CTA, keys per KV tile, head dim
+constexpr int ATT_HALF_BYTES = 128 * 128;  // one 64-column half of a 128x128 bf16 tile
+constexpr int ATT_TILE_BYTES = 2 * ATT_HALF_BYTES;
+constexpr int ATT_STAGES = 2;
+constexpr int ATT_SMEM = ATT_TILE_BYTES + ATT_STAGES * 2 * ATT_TILE_BYTES + 256 + 1024;
+
+struct AttnParams {
+  int Lq, Lk, heads;
+  int ldo;
+  int vt_chunk_len;
+  __nv_bfloat16* O;
+  float scale_log2;             // softmax scale * log2(e)
+  const uint32_t* chunk_flags;  // context-parallel gate (or NULL): chunk c readable once chunk_flags[c] >= flag_seq
+  uint32_t flag_seq;
+  int first_chunk;
+  unsigned long long peer_timeout_ns;  // bound of the wait for a peer's chunk flag (and of this CTA's barrier waits
+                                       // while such a wait may be pending): an inter-process dependency, not a protocol bug
+  unsigned long long* wait_ns;         // optional profiling counter: ns spent polling chunk flags, summed over CTAs
+  unsigned long long* trace;           // kTrace only: [3 roles][64 steps][8 slots] clock64 stamps of CTA (0,0)
+};
+
+static unsigned long long* g_attn_trace = nullptr;
+
+#define ATT_TR(role, slot)                                                                                  \
+  do {                                                                                                      \
+    if constexpr (kTrace) {                                                                                 \
+      if (blockIdx.x == 0 && blockIdx.y == 0 && j < 64 && (threadIdx.x % 128) == 0)                         \
+        p.trace[((role) * 64 + j) * 8 + (slot)] = clock64();                                                \
+    }                                                                                                       \
+  } while (0)
+
+__device__ __forceinline__ float ex2_approx(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;\n" : "=f"(y) : "f"(x));
+  return y;
+}
+
+template <bool kTrace>
+__global__ void __launch_bounds__(ATT_THREADS, 1)
+    k_attn_fwd(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+               const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  uint8_t* smem_q = smem;
+  uint8_t* smem_k = smem + ATT_TILE_BYTES;                          // [ATT_STAGES] K tiles
+  uint8_t* smem_v = smem_k + ATT_STAGES * ATT_TILE_BYTES;            // [ATT_STAGES] V^T tiles
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_v + ATT_STAGES * ATT_TILE_BYTES);
+  uint64_t* q_full = bars;                        // [1]
+  uint64_t* k_full = bars + 1;                    // [ATT_STAGES]
+  uint64_t* v_full = bars + 1 + ATT_STAGES;       // [ATT_STAGES]
+  uint64_t* kv_empty = bars + 1 + 2 * ATT_STAGES; // [ATT_STAGES]
+
+  const uint32_t wg = threadIdx.x / 128;
+  const uint32_t tid = threadIdx.x % 128;
+  const int head = blockIdx.y;
+  const int q0 = blockIdx.x * ATT_TILE;
+  const int n_kv = p.Lk / ATT_TILE;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmQ);
+    tma_prefetch_desc(&tmK);
+    tma_prefetch_desc(&tmV);
+    mbar_init(q_full, 1);
+    for (int i = 0; i < ATT_STAGES; ++i) {
+      mbar_init(&k_full[i], 1);
+      mbar_init(&v_full[i], 1);
+      mbar_init(&kv_empty[i], 2);  // one arrive per consumer warpgroup
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    // ===== TMA producer =====
+    setmaxnreg_dec<24>();
+    if (tid == 0) {
+      mbar_expect_tx(q_full, ATT_TILE_BYTES);
+      for (int h = 0; h < 2; ++h) tma_load_2d(smem_q + h * ATT_HALF_BYTES, &tmQ, q_full, head * 128 + h * 64, q0);
+      const int tiles_per_chunk = p.vt_chunk_len / ATT_TILE;
+      const int n_chunks = p.Lk / p.vt_chunk_len;
+      uint32_t stage = 0, phase = 0;
+      for (int j = 0; j < n_kv; ++j) {
+        // KV tiles are visited chunk by chunk starting with `first_chunk` (the local one under context
+        // parallelism); a remote chunk is only touched after its producer rank has published it.
+        int chunk = p.first_chunk + j / tiles_per_chunk;
+        if (chunk >= n_chunks) chunk -= n_chunks;
+        const int within = j % tiles_per_chunk;
+        if (p.chunk_flags && within == 0 && chunk != p.first_chunk) {  // the local chunk is ordered by the stream
+          uint32_t v, spins = 0;
+          uint64_t t0 = 0;
+          for (;;) {
+            asm volatile("ld.acquire.sys.global.u32 %0, [%1];\n" : "=r"(v) : "l"(p.chunk_flags + chunk) : "memory");
+            if ((int)(v - p.flag_seq) >= 0) break;
+            if (t0 == 0) t0 = global_timer_ns();
+            if ((++spins & 0x3FFu) == 0 && global_timer_ns() - t0 > p.peer_timeout_ns) asm volatile("trap;\n");
+          }
+          if (t0 != 0 && p.wait_ns) atomicAdd(p.wait_ns, (unsigned long long)(global_timer_ns() - t0));
+          asm volatile("fence.proxy.async.global;\n" ::: "memory");  // peer-written data is read by the TMA next
+        }
+        const int kv0 = chunk * p.vt_chunk_len + within * ATT_TILE;
+        mbar_wait_ns(&kv_empty[stage], phase ^ 1, p.peer_timeout_ns);
+        mbar_expect_tx(&k_full[stage], ATT_TILE_BYTES);
+        for (int h = 0; h < 2; ++h)  // the two 64-dim halves of 128 keys
+          tma_load_2d(smem_k + stage * ATT_TILE_BYTES + h * ATT_HALF_BYTES, &tmK, &k_full[stage], head * 128 + h * 64,
+                      kv0);
+        mbar_expect_tx(&v_full[stage], ATT_TILE_BYTES);
+        for (int h = 0; h < 2; ++h)  // the two 64-key halves of 128 head dimensions
+          tma_load_3d(smem_v + stage * ATT_TILE_BYTES + h * ATT_HALF_BYTES, &tmV, &v_full[stage],
+                      within * ATT_TILE + h * 64, head * 128, chunk);
+        if (++stage == ATT_STAGES) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+    }
+  } else {
+    // ===== consumers: warpgroup c owns query rows [64c, 64c + 64) of the tile =====
+    setmaxnreg_inc<240>();
+    const uint32_t c = wg - 1;
+    const uint32_t warp = tid / 32, lane = tid % 32;
+    // accumulator layout (wgmma m64n128k16, f32), i in [0, 16): acc[4i + {0,1}] = row 16 warp + lane/4, columns 8i + 2 (lane%4) + {0,1};
+    // acc[4i + {2,3}] = the same columns eight rows further down
+    float o[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) o[i] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY};  // running row max (log2 units) of the two rows of this thread
+    float l_run[2] = {0.f, 0.f};              // this thread's partial row sums (quad-reduced at the end)
+    const float sl2 = p.scale_log2;
+    const uint64_t dq = make_sdesc_sw128(smem_u32(smem_q + c * 64 * 128));
+    mbar_wait_ns(q_full, 0, p.peer_timeout_ns);
+    uint32_t stage = 0, phase = 0;
+    for (int j = 0; j < n_kv; ++j) {
+      ATT_TR(1 + c, 0);
+      float s[64];
+      mbar_wait_ns(&k_full[stage], phase, p.peer_timeout_ns);
+      ATT_TR(1 + c, 1);
+      {
+        const uint64_t dk = make_sdesc_sw128(smem_u32(smem_k + stage * ATT_TILE_BYTES));
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk) {  // head dimensions 16 kk .. 16 kk + 15
+          const uint32_t off = (kk >> 2) * ATT_HALF_BYTES + (kk & 3) * 32;
+          wgmma_ss_n128(s, sdesc_advance(dq, off), sdesc_advance(dk, off), kk > 0 ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(s);
+      }
+      ATT_TR(1 + c, 2);
+      // ---- online softmax (exact row max of every tile) ----
+      float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        mx[0] = fmaxf(mx[0], fmaxf(s[4 * i], s[4 * i + 1]));
+        mx[1] = fmaxf(mx[1], fmaxf(s[4 * i + 2], s[4 * i + 3]));
+      }
+      float alpha[2], nm[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+        nm[h] = fmaxf(m_run[h], mx[h] * sl2);
+        alpha[h] = ex2_approx(m_run[h] - nm[h]);  // 0 on the first tile (m_run = -inf)
+        m_run[h] = nm[h];
+        l_run[h] *= alpha[h];
+      }
+      uint32_t pa[32];  // P as bf16 pairs: the A fragments of the 8 k-steps of P V
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const float p0 = ex2_approx(fmaf(s[4 * i], sl2, -nm[0])), p1 = ex2_approx(fmaf(s[4 * i + 1], sl2, -nm[0]));
+        const float p2 = ex2_approx(fmaf(s[4 * i + 2], sl2, -nm[1])), p3 = ex2_approx(fmaf(s[4 * i + 3], sl2, -nm[1]));
+        l_run[0] += p0 + p1;
+        l_run[1] += p2 + p3;
+        pa[2 * i] = pack_bf16x2(p0, p1);
+        pa[2 * i + 1] = pack_bf16x2(p2, p3);
+      }
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        o[4 * i] *= alpha[0];
+        o[4 * i + 1] *= alpha[0];
+        o[4 * i + 2] *= alpha[1];
+        o[4 * i + 3] *= alpha[1];
+      }
+      ATT_TR(1 + c, 3);
+      // ---- O += P V_j ----
+      mbar_wait_ns(&v_full[stage], phase, p.peer_timeout_ns);
+      {
+        const uint64_t dv = make_sdesc_sw128(smem_u32(smem_v + stage * ATT_TILE_BYTES));
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk) {  // keys 16 kk .. 16 kk + 15 = accumulator columns of S
+          const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
+          wgmma_rs_n128(o, a, sdesc_advance(dv, (kk >> 2) * ATT_HALF_BYTES + (kk & 3) * 32));
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(o);
+      }
+      if (tid == 0) mbar_arrive(&kv_empty[stage]);
+      ATT_TR(1 + c, 4);
+      if (++stage == ATT_STAGES) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    // ---- normalise and store ----
+    float inv[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float l = l_run[h];
+      l += __shfl_xor_sync(0xffffffffu, l, 1);
+      l += __shfl_xor_sync(0xffffffffu, l, 2);
+      inv[h] = 1.0f / l;
+    }
+    const int row_a = q0 + (int)(c * 64 + warp * 16 + lane / 4);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = row_a + 8 * h;
+      if (row >= p.Lq) continue;
+      __nv_bfloat16* dst = p.O + (size_t)row * p.ldo + head * 128 + 2 * (lane % 4);
+#pragma unroll
+      for (int i = 0; i < 16; ++i)
+        *reinterpret_cast<uint32_t*>(dst + 8 * i) = pack_bf16x2(o[4 * i + 2 * h] * inv[h], o[4 * i + 2 * h + 1] * inv[h]);
+    }
+  }
+}
+
+int attn_fwd(const void* q, const void* k, const void* vt, void* o, int Lq, int Lk, int heads,
+             int ldq, int ldk, int ldo, int vt_chunk_len, float scale, cudaStream_t st, const ChunkGate* gate) {
+  G3C_REQUIRE(q && k && vt && o, "attn: null operand");
+  G3C_REQUIRE(Lq > 0 && Lk > 0 && heads > 0, "attn: bad sizes");
+  G3C_REQUIRE(Lk % ATT_TILE == 0, "attn: Lk=%d must be a multiple of 128", Lk);
+  if (vt_chunk_len <= 0) vt_chunk_len = Lk;
+  G3C_REQUIRE(Lk % vt_chunk_len == 0 && vt_chunk_len % ATT_TILE == 0,
+              "attn: vt_chunk_len=%d must divide Lk=%d and be a multiple of 128", vt_chunk_len, Lk);
+  G3C_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldo % 8 == 0 && ldq >= heads * 128 &&
+                  ldk >= heads * 128 && ldo >= heads * 128,
+              "attn: leading dimensions must be >= heads*128 and multiples of 8");
+  G3C_REQUIRE((reinterpret_cast<uintptr_t>(o) & 15) == 0, "attn: O must be 16-byte aligned");
+  CUtensorMap tmQ, tmK, tmV;
+  {
+    uint64_t dims[2] = {(uint64_t)heads * 128, (uint64_t)Lq}, str[1] = {(uint64_t)ldq * 2};
+    uint32_t box[2] = {64, 128};
+    int rc = make_tmap_bf16_sw128(&tmQ, q, 2, dims, str, box);
+    if (rc) return rc;
+  }
+  {
+    uint64_t dims[2] = {(uint64_t)heads * 128, (uint64_t)Lk}, str[1] = {(uint64_t)ldk * 2};
+    uint32_t box[2] = {64, 128};
+    int rc = make_tmap_bf16_sw128(&tmK, k, 2, dims, str, box);
+    if (rc) return rc;
+  }
+  {
+    const int chunks = Lk / vt_chunk_len;
+    uint64_t dims[3] = {(uint64_t)vt_chunk_len, (uint64_t)heads * 128, (uint64_t)chunks};
+    uint64_t str[2] = {(uint64_t)vt_chunk_len * 2, (uint64_t)vt_chunk_len * 2 * heads * 128};
+    uint32_t box[3] = {64, 128, 1};
+    int rc = make_tmap_bf16_sw128(&tmV, vt, 3, dims, str, box);
+    if (rc) return rc;
+  }
+  static bool configured = false;
+  if (!configured) {
+    G3C_CUDA(cudaFuncSetAttribute(k_attn_fwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
+    G3C_CUDA(cudaFuncSetAttribute(k_attn_fwd<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
+    configured = true;
+  }
+  AttnParams p;
+  p.Lq = Lq;
+  p.Lk = Lk;
+  p.heads = heads;
+  p.ldo = ldo;
+  p.vt_chunk_len = vt_chunk_len;
+  p.O = reinterpret_cast<__nv_bfloat16*>(o);
+  // scale = ln 2 declares that Q already carries softmax scale * log2(e): S is then in log2 units
+  p.scale_log2 = scale * 1.4426950408889634f;
+  if (fabsf(p.scale_log2 - 1.0f) < 1e-6f) p.scale_log2 = 1.0f;
+  p.chunk_flags = gate ? gate->flags : nullptr;
+  p.peer_timeout_ns = gate ? peer_timeout_ns() : G3C_MBAR_TIMEOUT_NS;
+  p.wait_ns = gate ? gate->wait_ns : nullptr;
+  p.flag_seq = gate ? gate->seq : 0;
+  p.first_chunk = gate ? gate->first : 0;
+  p.trace = g_attn_trace;
+  G3C_REQUIRE(p.first_chunk >= 0 && p.first_chunk < Lk / vt_chunk_len, "attn: first chunk %d out of range", p.first_chunk);
+  dim3 grid((Lq + ATT_TILE - 1) / ATT_TILE, heads);
+  if (g_attn_trace) k_attn_fwd<true><<<grid, ATT_THREADS, ATT_SMEM, st>>>(tmQ, tmK, tmV, p);
+  else k_attn_fwd<false><<<grid, ATT_THREADS, ATT_SMEM, st>>>(tmQ, tmK, tmV, p);
+  G3C_CUDA(cudaGetLastError());
+  return G3C_OK;
+}
+
+}  // namespace g3c
+
+extern "C" int g3c_attn_set_trace(unsigned long long* device_buffer) {
+  g3c::g_attn_trace = device_buffer;
+  return G3C_OK;
+}
+
+extern "C" int g3c_attn_fwd(const void* q, const void* k, const void* vt, void* o, int Lq, int Lk,
+                            int heads, int ldq, int ldk, int ldo, int vt_chunk_len, float scale,
+                            void* stream) {
+  return g3c::attn_fwd(q, k, vt, o, Lq, Lk, heads, ldq, ldk, ldo, vt_chunk_len, scale,
+                       (cudaStream_t)stream, nullptr);
+}

@@ -1,6 +1,6 @@
-// Shared device-side primitives for the sm_100a kernels of gen3c_b200:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / st / fences),
-// UMMA shared-memory + instruction descriptors.  Raw PTX only; no CUTLASS dependency.
+// Shared device-side primitives for the sm_90a kernels of gen3c_b200:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (fences / groups / shared-memory descriptors).
+// Raw PTX only; no CUTLASS dependency.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -9,6 +9,7 @@
 #include <stdio.h>
 
 #include "../../include/gen3c_b200.h"
+#include "wgmma_ops.cuh"
 
 namespace g3c {
 
@@ -82,7 +83,7 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 }
 // G3C_MBAR_SUSPEND_NS: suspend-time hint of mbarrier.try_wait — the thread may sleep that long before the instruction
 // returns false (it still wakes as soon as the phase completes), so a waiting warp re-issues the poll loop less often.
-// Measured with 20 us on the attention kernel: 1 219 / 1 241 against 1 240 / 1 255 TFLOP/s without — off by default.
+// Off by default.
 #ifndef G3C_MBAR_SUSPEND_NS
 #define G3C_MBAR_SUSPEND_NS 0
 #endif
@@ -119,7 +120,7 @@ __device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Spin with a generous bound so that a protocol bug traps instead of hanging the GPU box.
+// Spin with a generous bound so that a protocol bug traps instead of hanging the GPU.
 #ifndef G3C_MBAR_TIMEOUT_NS
 #define G3C_MBAR_TIMEOUT_NS 4000000000ull
 #endif
@@ -128,7 +129,7 @@ __device__ __forceinline__ uint64_t global_timer_ns() {
   asm volatile("mov.u64 %0, %%globaltimer;\n" : "=l"(t));
   return t;
 }
-// A protocol bug must trap instead of hanging the GPU box.  No function call / printf here: a call inside a
+// A protocol bug must trap instead of hanging the GPU.  No function call / printf here: a call inside a
 // setmaxnreg region forces ptxas to size the whole kernel for the smallest register budget.
 #ifdef G3C_MBAR_DEBUG
 #define G3C_MBAR_TIMEOUT_ACTION(bar, parity)                                                                 \
@@ -216,79 +217,31 @@ __device__ __forceinline__ void tma_store_wait_all() {
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, fences, MMA, commit, ld/st
+// wgmma (Hopper warpgroup MMA): fences, groups, shared-memory descriptors
 // ----------------------------------------------------------------------------------------------
-// Whole warp must call.  ncols: power of two in [32, 512].
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(
-                   smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-}
-__device__ __forceinline__ void tc_wait_ld() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void tc_wait_st() {
-  asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory");
+// The accumulators of an asynchronous wgmma are written behind the compiler's back: pin every register read or written
+// around it to this point of the instruction stream (after wgmma_wait, before the next wgmma).
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
 
-// D[tmem] (+)= A[smem] * B[smem]^T   (both K-major), bf16 in, fp32 accumulate.
-__device__ __forceinline__ void umma_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                        uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]^T   (A: lane = row m, 16-bit elements packed two per column).
-__device__ __forceinline__ void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b,
-                                        uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives once all tcgen05 ops previously issued by this thread have completed.
-// (implies tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-
-// UMMA instruction descriptor: kind::f16, A=B=bf16, D=f32, both operands K-major.
-// Bit layout (cute::UMMA::InstrDescriptor): c_format[4,6)=1(F32) a_format[7,10)=1(BF16)
-// b_format[10,13)=1 a_major[15]=0 b_major[16]=0 n_dim[17,23)=N>>3 m_dim[24,29)=M>>4.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor for a K-major tile stored with the 128-byte swizzle
-// (rows of 64 bf16 = 128 B, 8-row groups 1024 B apart, tile base 1024-B aligned):
-// start_address[0,14) = addr>>4, LBO[16,30) = 0 (unused for swizzled K-major),
-// SBO[32,46) = 1024>>4, version[46,48) = 1 (sm_100), layout_type[61,64) = 2 (SWIZZLE_128B).
+// Shared-memory matrix descriptor of a K-major tile stored with the 128-byte swizzle (rows of 64 bf16 = 128 B, 8-row
+// groups 1024 B apart, tile base 1024-B aligned): start_address[0,14) = addr>>4, LBO[16,30) (unused for swizzled
+// K-major), SBO[32,46) = 1024>>4, layout_type[62,64) = 1 (SWIZZLE_128B).
 __device__ __forceinline__ uint64_t make_sdesc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
+  d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(1024u >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 // advance along K inside the 128-byte swizzle span: +bytes on the (unswizzled) start address
@@ -296,158 +249,14 @@ __device__ __forceinline__ uint64_t sdesc_advance(uint64_t d, uint32_t bytes) {
   return d + static_cast<uint64_t>(bytes >> 4);
 }
 
-// TMEM -> registers: each thread of the warp reads 32 consecutive fp32 columns of its own lane
-// (warp w may only touch lanes [32*(w%4), 32*(w%4)+32)).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+// Register budget of a warpgroup (all 128 threads execute it): producers give registers back, MMA warpgroups take them.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(N));
 }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n" ::"r"(
-          taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-      "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]),
-      "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]),
-      "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]),
-      "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-
-// 16-column variants (a quarter of a 128-key P row: 32 keys as bf16 pairs)
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-
-// ----------------------------------------------------------------------------------------------
-// CTA pairs (cta_group::2): two CTAs of a cluster on one TPC issue one 256-row UMMA and share the B operand
-// ----------------------------------------------------------------------------------------------
-// In a cluster, a shared::cta address is also a valid shared::cluster address of the executing CTA; clearing
-// bit 24 turns it into the address of the same offset in the EVEN CTA of the pair (the MMA leader).
-constexpr uint32_t kLeaderCtaMask = 0xFEFFFFFFu;
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
-}
-// TMA load into this CTA's shared memory; the transaction bytes are credited to the LEADER CTA's mbarrier
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];\n" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kLeaderCtaMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_2sm(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                                int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];\n" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kLeaderCtaMask), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2sm(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                                int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];\n" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kLeaderCtaMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-// arrive on the barrier at this offset in the leader CTA (a local arrive when executed by the leader itself)
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];\n" ::"r"(smem_u32(bar) & kLeaderCtaMask) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem, 256 rows over the CTA pair] (+)= A * B^T ; issued by ONE thread of the leader CTA
-__device__ __forceinline__ void umma_ss_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem, 256 rows over the CTA pair] (+)= A[tmem of each CTA] * B^T ; A: 16-bit elements packed two per column
-__device__ __forceinline__ void umma_ts_2sm(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit: arrive on the mbarrier at this offset in BOTH CTAs of the pair once the prior MMAs are done
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n" ::"r"(
-          smem_u32(bar)),
-      "h"((uint16_t)3)
-      : "memory");
-}
-
-// TMA load multicast to the CTAs of `mask`: the tile lands at the same CTA-relative offset in each destination and
-// credits the bytes to the mbarrier at the same offset in each destination.
-__device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                               uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%3, %4}], [%2], %5;\n" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_mc(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                               int c2, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%3, %4, %5}], [%2], %6;\n" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "h"(mask)
-      : "memory");
-}
-// commit of 1-CTA MMAs that arrives on the mbarrier at this offset in every CTA of `mask`
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-// store a 32-bit value at this CTA-relative shared-memory offset in CTA `rank` of the cluster
-__device__ __forceinline__ void st_shared_cluster_u32(const void* local_ptr, uint32_t rank, uint32_t v) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;\n" : "=r"(remote) : "r"(smem_u32(local_ptr)), "r"(rank));
-  asm volatile("st.shared::cluster.u32 [%0], %1;\n" ::"r"(remote), "r"(v) : "memory");
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(N));
 }
 
 // ----------------------------------------------------------------------------------------------

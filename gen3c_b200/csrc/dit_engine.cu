@@ -354,7 +354,7 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
   const int Lk_all = L * h->cp_size;
   const float attn_scale = 0.6931471805599453f;  // ln 2: 1/sqrt(128) * log2(e) is folded into the query RMSNorm gain
   // to_q / to_k: Linear + per-head RMSNorm (+ RoPE).  Fused into the GEMM epilogue (G3C_FUSE_NORM_ROPE, default on):
-  // the norm and the rotation act on the fp32 accumulators in TMEM and the [tokens, D] bf16 round trip of a separate
+  // the norm and the rotation act on the fp32 accumulators in registers and the [tokens, D] bf16 round trip of a separate
   // pass disappears.
   static int fuse_nr = -1;
   if (fuse_nr < 0) {

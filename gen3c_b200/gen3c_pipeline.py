@@ -92,7 +92,7 @@ class Gen3cPipeline:
         if not disable_guardrail:
             raise NotImplementedError("the guardrail models are outside this engine's scope: pass --disable_guardrail")
         if offload_network or offload_tokenizer or offload_text_encoder_model:
-            raise NotImplementedError("model offloading is unnecessary on a 180 GB B200 and is not implemented")
+            raise NotImplementedError("model offloading is not implemented (the 7B DiT and its workspace fit one 80 GB H100)")
         self.inference_type, self.checkpoint_dir, self.checkpoint_name = inference_type, checkpoint_dir, checkpoint_name
         self.model_name = checkpoint_name
         self.enable_prompt_upsampler, self.disable_guardrail = enable_prompt_upsampler, disable_guardrail

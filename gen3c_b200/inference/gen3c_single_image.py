@@ -1,4 +1,4 @@
-"""Single-image GEN3C generation — the reference's command-line entry point on the B200-native engine.
+"""Single-image GEN3C generation — the reference's command-line entry point on the H100-native engine.
 
 reference: cosmos_predict1/diffusion/inference/gen3c_single_image.py — create_parser :35-99, validate_args :106-108,
 _predict_moge_depth :110-203, _predict_moge_depth_from_tensor :205-221, demo :223-477.  Same argparse surface (plus

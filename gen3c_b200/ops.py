@@ -19,7 +19,7 @@ def _chk(t: torch.Tensor, dtype, name: str):
 
 def gemm(a: torch.Tensor, b: torch.Tensor, epilogue: int = EPI_BF16, out: Optional[torch.Tensor] = None,
          gate: Optional[torch.Tensor] = None, block_n: int = 0) -> torch.Tensor:
-    """out[M,N] = a[M,K] @ b[N,K]^T on tcgen05 (bf16 in, fp32 accumulate).
+    """out[M,N] = a[M,K] @ b[N,K]^T on wgmma (bf16 in, fp32 accumulate).
     epilogue: EPI_BF16 | EPI_GELU_BF16 (bf16 out) | EPI_F32 (f32 out) | EPI_GATED_RESIDUAL_F32 (out f32 += gate*acc)."""
     _chk(a, torch.bfloat16, "a")
     _chk(b, torch.bfloat16, "b")

@@ -8,7 +8,7 @@ and `encode` / `decode` / `get_latent_num_frames` / `get_pixel_num_frames` behav
 
 As in the reference the convolutional encoder / decoder themselves are the TorchScript modules shipped in
 `checkpoints/Cosmos-Tokenize1-CV8x8x8-720p/{encoder,decoder}.jit` and executed by torch — they are data, not code of
-either repository.  A native sm_100a VAE is outside this round's scope (DESIGN.md §6); this wrapper is what lets the
+either repository.  A native sm_90a VAE is outside this round's scope (DESIGN.md §6); this wrapper is what lets the
 entry point (`gen3c_b200/inference/gen3c_single_image.py`) run the real tokenizer when the checkpoint directory exists.
 `SyntheticVideoTokenizer` is a weight-free stand-in with the same interface and compression factors for tests and the
 synthetic end-to-end run; it is only used when the caller asks for it by name.

@@ -1,5 +1,5 @@
 /*
- * gen3c_b200 — C ABI of libgen3c_b200.so (sm_100a).
+ * gen3c_b200 — C ABI of libgen3c_b200.so (sm_90a, H100).
  *
  * The reference (nv-tlabs/GEN3C) has no FFI: its seams are Python call sites.  Each entry point
  * below replaces one of them; the citation is the reference file:line whose arithmetic it
@@ -118,7 +118,7 @@ int g3c_render_cache_occlusion(const float* points, const unsigned char* boundar
 #define G3C_EPI_GATED_RESIDUAL_F32 2 /* D (f32) += gate[n] * acc                */
 #define G3C_EPI_F32 3                /* D (f32) = acc                           */
 
-/* D[M,N] = A[M,K] . B[N,K]^T, bf16 operands (K contiguous), fp32 accumulation on tcgen05/TMEM.
+/* D[M,N] = A[M,K] . B[N,K]^T, bf16 operands (K contiguous), fp32 accumulation on wgmma (Hopper tensor cores).
  * Replaces every nn.Linear of the net (reference: module/attention.py:263-266,289,91-102;
  * module/blocks.py:153-163,228-241).  block_n: 0 = auto, or 64/128/256. */
 int g3c_gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, int lda, int ldb,
@@ -139,13 +139,14 @@ int g3c_gemm_norm_rope_bf16(const void* A, const void* B, void* D, int M, int N,
  *   Lk must be a multiple of 128.
  *   scale = ln 2 (0.6931472) declares that Q already carries softmax_scale * log2(e) (the DiT engine folds it into
  *   the query RMSNorm gain): the scores are then exponentiated as 2^s without a multiply per score.
- *   block_n of g3c_gemm_bf16: 512 selects the CTA-pair kernel (256 x 256 tile), 0 chooses by wave count. */
+ *   block_n of g3c_gemm_bf16: 0 chooses (256 when N % 256 == 0, else 128 or 64); 512 is accepted and runs 256. */
 int g3c_attn_fwd(const void* q, const void* k, const void* vt, void* o, int Lq, int Lk, int heads,
                  int ldq, int ldk, int ldo, int vt_chunk_len, float scale, void* stream);
 
 /* Profiling aid: when a device buffer of 3*64*8 uint64 is registered, the next g3c_attn_fwd launches run a
- * traced build of the kernel in which CTA (0,0) records clock64() stamps per KV step: role 0 = MMA issuer,
- * 1/2 = softmax tile A/B.  NULL switches tracing off.  (tools/attn_trace.py prints the timeline.) */
+ * traced build of the kernel in which CTA (0,0) records clock64() stamps per KV step (first 64 steps): roles 1/2 = the
+ * two consumer warpgroups; slots 0 step start, 1 K landed, 2 S = Q K^T done, 3 softmax done, 4 P V done.  NULL
+ * switches tracing off. */
 int g3c_attn_set_trace(unsigned long long* device_buffer);
 
 /* x (f32 [L,D]) += pos (bf16, optional) ; y (bf16) = LayerNorm_eps(x) * (1 + scale) + shift

@@ -13,7 +13,7 @@ import sys
 import numpy as np
 import torch
 
-from . import cases, dit_oracle, ref_stubs, warp_oracle
+from . import cases, dit_oracle, golden, ref_stubs, warp_oracle
 
 OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden")
 
@@ -53,7 +53,7 @@ def mint_warp():
         rce = torch.minimum(torch.clamp(rce, min=0), lim)
         idx_equal = bool((t(fl) == rfl).all() and (t(ce) == rce).all())
         report.append((name, e_pts, e_img, e_msk, e_dep, e_flow, idx_equal, float(mask.mean())))
-        np.savez_compressed(os.path.join(OUT, f"warp_{name}.npz"), points=pts.numpy(), warped=warped.numpy(),
+        golden.save(OUT, f"warp_{name}", points=pts.numpy(), warped=warped.numpy(),
                             mask=mask.numpy(), depth=depth.numpy(), flow=flow.numpy(),
                             floor=rfl.numpy().astype(np.int32), ceil=rce.numpy().astype(np.int32))
     # reliability mask + render_cache chunking through the reference's Cache3D_Buffer (N = 2 buffers)
@@ -76,7 +76,7 @@ def mint_warp():
     m2 = cache.input_mask.numpy()[:, :, :, 0].astype(np.float32)
     pix_o, msk_o = warp_oracle.render_cache(pts2, img2, m2, w2cs.numpy(), Ks.numpy())
     e_cache = float(np.abs(pix_o - pix.numpy()).max())
-    np.savez_compressed(os.path.join(OUT, "warp_cache.npz"), pixels=pix.numpy(), masks=msk.numpy(),
+    golden.save(OUT, "warp_cache", pixels=pix.numpy(), masks=msk.numpy(),
                         reliable=rel.numpy(), points=pts2, cache_mask=m2)
     print("== Path R: restated oracle vs reference (max abs err) ==")
     for r in report:
@@ -137,7 +137,7 @@ def mint_foreground(ref):
     print("Path R foreground masking (R7): boundary px %.3f, occluded px %.4f, oracle mask flips %.2e, image err %.2e, "
           "boundary mask equal: %s" % (float(boundary.float().mean()), killed, flips, e_img,
                                        bool((b_o == boundary.numpy()).all())))
-    np.savez_compressed(os.path.join(OUT, "warp_R7_foreground.npz"), points=pts.numpy(), boundary=boundary.numpy(),
+    golden.save(OUT, "warp_R7_foreground", points=pts.numpy(), boundary=boundary.numpy(),
                         warped=warped.numpy(), mask=mask.numpy(), depth=depth.numpy(), mask_plain=base[1].numpy())
     return 0 if (killed > 0.005 and flips < 2e-3 and e_img < 2e-3) else 1
 
@@ -191,7 +191,7 @@ def mint_dit():
     net_bf = net_bf.to(torch.bfloat16).eval()
     out_c_bf = run(net_bf, torch.bfloat16, inp["pose"], inp["ctx_c"])
     floor = rel(out_c_bf, out_c)
-    np.savez_compressed(os.path.join(OUT, "dit_tiny.npz"), out_cond=out_c.numpy(), out_uncond=out_u.numpy(),
+    golden.save(OUT, "dit_tiny", out_cond=out_c.numpy(), out_uncond=out_u.numpy(),
                         ref_bf16_rel_l2=np.float32(floor))
     print("== Path D (tiny 2-block, D=256, L=128): restated oracle vs reference fp32 forward ==")
     print("  rel-L2 cond %.2e  uncond %.2e ; reference bf16-vs-fp32 noise floor rel-L2 %.2e" % (e_c, e_u, floor))
@@ -295,7 +295,7 @@ def mint_cache_classes():
             w2, k2 = cu.generate_camera_trajectory(ty, w0, K[0], 7, 0.3, rot, center_depth=1.7, device="cpu")
             out[f"traj_{ty}_{rot}"] = w2.numpy()
     out["traj_w0"] = w0.numpy()
-    np.savez_compressed(os.path.join(OUT, "warp_cache_classes.npz"), **out)
+    golden.save(OUT, "warp_cache_classes", **out)
     # the restated oracle against the same runs
     po = warp_oracle.unproject_points(c6["depth"], c6["w2c_src"], c6["K"], is_depth=False)
     print("== Path R classes: ring/selector/4D/alignment goldens written; oracle unproject(is_depth=False) err %.2e; "
@@ -340,7 +340,7 @@ def mint_dit_fullwidth():
     ob = dit_oracle.forward({k: v.to(torch.bfloat16) for k, v in sd.items()}, cfg, inp["x"], inp["cond_mask"], inp["pose"],
                             inp["padding"], inp["timestep"], inp["ctx_c"], compute_dtype=torch.bfloat16).float()
     eb = float((ob - out).norm() / out.norm())
-    np.savez_compressed(os.path.join(OUT, "dit_fullwidth.npz"), out_cond=out.numpy(), oracle_bf16_rel_l2=np.float32(eb))
+    golden.save(OUT, "dit_fullwidth", out_cond=out.numpy(), oracle_bf16_rel_l2=np.float32(eb))
     print("== Path D (1 block at full width D=4096/32 heads/ffn 16384/ctx 512x1024, 7 040 tokens): restated oracle vs the "
           "reference's fp32 forward rel-L2 %.2e ; bf16 run of the oracle vs it %.2e ==" % (e, eb))
     return 0 if e < 1e-4 else 1
@@ -371,7 +371,7 @@ def mint_tokenizer():
             out[f"z_{tag}"], out[f"y_{tag}"] = z.float().numpy(), y.float().numpy()
             out["frames"] = np.array([tok.get_latent_num_frames(1), tok.get_latent_num_frames(34), tok.get_pixel_num_frames(6),
                                       tok.latent_chunk_duration])
-    np.savez_compressed(os.path.join(OUT, "vae_wrapper.npz"), **out)
+    golden.save(OUT, "vae_wrapper", **out)
     print("== tokenizer wrapper golden written: latent", out["z_f32"].shape, "video", out["y_f32"].shape, "==")
     return 0
 

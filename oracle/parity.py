@@ -1,5 +1,5 @@
 """ORACLE (test infrastructure only) — engine-vs-oracle comparison of the DiT forward at BASELINE width, shared by
-tests/test_fullsize_parity_gpu.py and tools/parity_report.py.  Needs a CUDA device: the fp32 oracle graph
+tests/test_fullsize_parity_gpu.py.  Needs a CUDA device: the fp32 oracle graph
 (oracle/dit_oracle.py, TF32 off, explicit fp32 attention) runs on the GPU next to the engine, on the same weights.
 
 What is measured, per depth (number of FA-CA-MLP blocks, final layer always applied):

@@ -2,7 +2,7 @@
 CPU by faking the third-party packages that are absent from this container (SURVEY.md Appendix A).
 
 Only used by ``oracle/make_golden.py`` (in the build container, where /root/reference exists) to mint
-the golden vectors under ``tests/golden/``.  Nothing here runs on the GPU box.
+the golden vectors under ``tests/golden/``.  Nothing here runs on the GPU.
 
 Restated third-party semantics (not in /root/reference; pins from the reference's INSTALL.md /
 requirements.txt): transformer-engine 1.12.0 RMSNorm / apply_rotary_pos_emb / DotProductAttention,

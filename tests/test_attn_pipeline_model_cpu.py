@@ -1,7 +1,10 @@
-"""Discrete-event model of the barrier protocol of k_attn_fwd1t (gen3c_b200/csrc/attn_tcgen05.cu): one query tile per CTA,
-kBufs S buffers in TMEM, a ring of {K_{j+kBufs}, V_j} stages, S(j+kBufs) issued behind P.V(j).
+"""Discrete-event model of a software-pipelined attention barrier protocol with S lookahead: one query tile per CTA, kBufs
+S accumulator buffers, a ring of {K_{j+kBufs}, V_j} stages, S(j+kBufs) issued behind P.V(j) by a single MMA issuer.  The
+attention kernel (gen3c_b200/csrc/attn_wgmma.cu) does not pipeline S yet (each consumer warpgroup runs S -> softmax -> P.V
+in order, DESIGN.md §7); this model is the protocol that lookahead is to follow, and it is validated here before any
+kernel relies on it.
 
-The model restates the kernel's bookkeeping — ring slot / phase, per-buffer parity bits of the softmax warps (`sph`) and of the
+The model restates the protocol's bookkeeping — ring slot / phase, per-buffer parity bits of the softmax warps (`sph`) and of the
 issuer (`pph`), the prologue, the commits behind every P.V, the final waits, the second (exact) pass continuing with the same
 parities — and runs the roles (loader, issuer, softmax warps, in-order tensor pipe, asynchronous TMA) under random
 interleavings.  It checks what the hardware tests can only show by not hanging:

@@ -7,12 +7,12 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import cases, warp_oracle
+from oracle import cases, golden, warp_oracle
 
 
 @pytest.fixture(scope="module")
 def g(golden_dir):
-    return np.load(os.path.join(golden_dir, "warp_cache_classes.npz"))
+    return golden.load(golden_dir, "warp_cache_classes")
 
 
 def test_camera_trajectories_match_reference(g):

@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import cases
+from oracle import cases, golden
 
 pytestmark = pytest.mark.gpu
 
@@ -19,7 +19,7 @@ def cu(a):
 
 @pytest.fixture(scope="module")
 def g(golden_dir):
-    return np.load(os.path.join(golden_dir, "warp_cache_classes.npz"))
+    return golden.load(golden_dir, "warp_cache_classes")
 
 
 def same_render(pix, msk, ref_pix, ref_msk, atol=2e-3, flips=2e-3, frac=0.999):

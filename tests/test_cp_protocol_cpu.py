@@ -1,7 +1,7 @@
 """Properties of the context-parallel K/V exchange schedule (gen3c_b200/csrc/dit_engine.cu, default `p2p` mode), stated
 on a pure-Python model of the two loops that define it:
   producer `me` pushes its slice to peers (me-1), (me-2), ... (mod N), each push followed by that peer's flag;
-  consumer `c` (attn_tcgen05.cu, TMA warp) visits KV chunks c, c+1, c+2, ... (mod N), the local one ungated.
+  consumer `c` (attn_wgmma.cu, TMA producer) visits KV chunks c, c+1, c+2, ... (mod N), the local one ungated.
 The schedule is right when every consumer's k-th remote chunk is the k-th push of the rank that produces it, so that all
 ranks can consume chunk k after k transfer slots."""
 import pytest

@@ -8,12 +8,12 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import cases, dit_oracle, warp_oracle
+from oracle import cases, dit_oracle, golden, warp_oracle
 
 
 @pytest.mark.parametrize("name", ["R1", "R2", "R3", "R4", "R5", "R6"])
 def test_warp_oracle_matches_reference_golden(name, golden_dir):
-    g = np.load(os.path.join(golden_dir, f"warp_{name}.npz"))
+    g = golden.load(golden_dir, f"warp_{name}")
     c = cases.warp_case(name)
     pts = warp_oracle.unproject_points(c["depth"], c["w2c_src"], c["K"])
     np.testing.assert_allclose(pts, g["points"], atol=2e-5, rtol=1e-5)
@@ -32,7 +32,7 @@ def test_foreground_masking_oracle_matches_reference_golden(golden_dir):
     """SURVEY.md §8f rank 1 (next row): forward_warp(foreground_masking=True).  The golden comes from the reference's own
     forward_warp / points_to_mesh / get_camera_rays run on CPU; only the NVIDIA-Warp ray/triangle kernel is replaced by
     a torch restatement there (oracle/make_golden.py::torch_ray_triangle)."""
-    g = np.load(os.path.join(golden_dir, "warp_R7_foreground.npz"))
+    g = golden.load(golden_dir, "warp_R7_foreground")
     c = cases.foreground_case()
     boundary = ~warp_oracle.reliable_depth_mask_range_batch(c["depth"]).astype(bool)[:, 0]
     assert np.array_equal(boundary, g["boundary"])
@@ -92,7 +92,7 @@ def test_chunk_coupling_kat():
 
 
 def test_render_cache_oracle_matches_reference(golden_dir):
-    g = np.load(os.path.join(golden_dir, "warp_cache.npz"))
+    g = golden.load(golden_dir, "warp_cache")
     c = cases.warp_case("R3")
     F = 3
     w2cs = cases.pan_trajectory(F, 0.1)[None]
@@ -108,7 +108,7 @@ def test_render_cache_oracle_matches_reference(golden_dir):
 
 
 def test_dit_oracle_matches_reference_golden(golden_dir):
-    g = np.load(os.path.join(golden_dir, "dit_tiny.npz"))
+    g = golden.load(golden_dir, "dit_tiny")
     cfg, shp = cases.TINY, cases.TINY_SHAPE
     sd = dit_oracle.random_state_dict(cfg, seed=0)
     inp = cases.dit_inputs(cfg, **shp)

@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import cases, dit_oracle
+from oracle import cases, dit_oracle, golden
 
 pytestmark = pytest.mark.gpu
 
@@ -41,7 +41,7 @@ def run_net(net, inp, pose, ctx, T):
 
 
 def test_tiny_forward_matches_reference_golden(golden_dir):
-    g = np.load(os.path.join(golden_dir, "dit_tiny.npz"))
+    g = golden.load(golden_dir, "dit_tiny")
     cfg, shp = cases.TINY, cases.TINY_SHAPE
     sd = dit_oracle.random_state_dict(cfg, seed=0)
     net = build_net(cfg, sd)

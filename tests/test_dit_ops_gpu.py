@@ -35,7 +35,7 @@ def test_gemm_bf16(M, N, K, bn):
 @pytest.mark.parametrize("M,N,K", [(256, 256, 64), (512, 512, 4096), (1000, 4096, 1024), (4096, 7168, 256), (128, 256, 512),
                                    (7040, 4096, 4096)])
 def test_gemm_cta_pair(M, N, K):
-    """CTA-pair kernel (tcgen05.mma.cta_group::2, 256 x 256 tile over two SMs), selected with block_n = 512."""
+    """block_n = 512, the C ABI's request for the widest tile (256 columns per CTA), with every epilogue."""
     from gen3c_b200 import ops
 
     a, b = bf(M, K, seed=21), bf(N, K, seed=22, s=0.05)
@@ -76,7 +76,7 @@ def test_gemm_transposed_output_by_operand_swap():
 @pytest.mark.parametrize("M,N,K,rope", [(1000, 256, 512, True), (512, 4096, 1024, False), (4096, 4096, 512, True),
                                           (300, 128, 256, True)])
 def test_gemm_norm_rope(M, N, K, rope):
-    """Projection + per-head RMSNorm + RoPE in the GEMM epilogue (1-CTA and CTA-pair kernels) against the composition
+    """Projection + per-head RMSNorm + RoPE in the GEMM epilogue (128- and 256-column tiles) against the composition
     gemm (fp32 out) -> oracle RMSNorm / RoPE."""
     from gen3c_b200 import ops
     from oracle import dit_oracle
@@ -103,7 +103,7 @@ def sdpa_ref(q, k, v, heads):
     return o.permute(1, 0, 2).reshape(Lq, D)
 
 
-# Lk > 1024 runs the pipelined kernel (one query tile per CTA pair half, three S buffers): cover n_kv mod 3 in {0, 1, 2},
+# one to 55 KV tiles (n_kv odd and even against the two-stage K/V ring),
 # ragged Lq (rows of the last tile and whole padding CTAs masked at the store), an odd number of query tiles, and a
 # chunked V^T layout (the context-parallel K/V order)
 @pytest.mark.parametrize("Lq,Lk,heads,chunks", [(256, 128, 1, 1), (256, 512, 2, 1), (384, 1024, 2, 1),
@@ -124,8 +124,8 @@ def test_attention(Lq, Lk, heads, chunks):
 
 @pytest.mark.parametrize("Lk", [1024, 2048])
 def test_attention_peaked_softmax(Lk):
-    """Large logits: exercises the rescale of O (scores spread over ~+-40).  Lk <= 1024 runs the exact kernel (row max
-    per tile), longer key ranges the default one (reference shifted by the row sums)."""
+    """Large logits: exercises the rescale of O (scores spread over ~+-40) as the row max keeps growing over the
+    KV tiles."""
     from gen3c_b200 import ops
 
     heads, Lq = 1, 256
@@ -139,14 +139,12 @@ def test_attention_peaked_softmax(Lk):
 
 @pytest.mark.parametrize("jump", [4.0, 9.5])
 def test_attention_score_jump(jump):
-    """A block of keys far above everything before it, inside one KV tile.  jump=4: the tile's row sums reach ~2^65,
-    which the default softmax (reference exponent guarded by the row sums) absorbs by shifting the reference before
-    the next tile.  jump=9.5: 2^155 overflows fp32 inside that tile, so the CTA must repeat its sweep in the exact
-    (max-per-tile) mode.  Both must match the fp32 reference, and the exact mode is the same kernel with
-    G3C_ATTN_MODE=0."""
+    """A block of keys far above everything before it, inside one KV tile: exp of the jump relative to the earlier
+    tiles is ~2^65 (jump=4) or ~2^155 (jump=9.5, beyond fp32), so the running max, O and the row sums must be rescaled
+    at that tile without overflow.  Both must match the fp32 reference."""
     from gen3c_b200 import ops
 
-    heads, Lq, Lk = 2, 384, 2048  # > 1024 keys: the default (sum-guarded) kernel, not the short-range exact one
+    heads, Lq, Lk = 2, 384, 2048
     q, k, v = bf(Lq, heads * 128, seed=20, s=0.5), bf(Lk, heads * 128, seed=21, s=0.5), bf(Lk, heads * 128, seed=22)
     q[:, :128] = 1.0  # head 0: constant queries; head 1 stays random
     k[300:340, :128] = jump  # scores 128 * jump / sqrt(128) = 11.3 * jump nats above the rest, in KV tile 2
@@ -158,10 +156,10 @@ def test_attention_score_jump(jump):
 
 @pytest.mark.parametrize("first_key", [260, 330])
 def test_attention_score_jump_in_one_key_half(first_key):
-    """The default kernel exponentiates every 128-key tile with two warps per row (64 keys each).  A jump confined to the
-    lower (keys 260..291 = columns 4..35 of tile 2) or the upper (330..361 = columns 74..105) half makes only ONE of them
-    see its partial row sum exceed the guard: it must post the shift so that both halves (and both halves of O) move to
-    the same reference before the next tile."""
+    """Each row of a 128-key tile is spread over the four threads of a quad (columns interleaved in groups of 8).  A jump
+    confined to the lower (keys 260..291 = columns 4..35 of tile 2) or the upper (330..361 = columns 74..105) half of
+    the tile is seen by part of each quad's columns only: the row max must be reduced over the whole quad so that every
+    column and all of O move to the same reference."""
     from gen3c_b200 import ops
 
     heads, Lq, Lk = 2, 384, 2048
@@ -177,8 +175,8 @@ def test_attention_score_jump_in_one_key_half(first_key):
 @pytest.mark.parametrize("gain", [1.0, 6.0])
 def test_attention_log2_units(gain):
     """scale = ln 2: the caller folded softmax_scale * log2(e) into Q (what the DiT engine does through the query
-    RMSNorm gain), so S arrives in log2 units.  gain=1: first-tile row maxima within 2^+-40 -> the fast tiles use
-    p = 2^s with no reference subtraction; gain=6: maxima beyond 2^40 -> the kernel keeps a reference exponent."""
+    RMSNorm gain), so S arrives in log2 units and the kernel exponentiates without a scale multiply.  gain=1: moderate
+    scores; gain=6: row maxima beyond 2^40."""
     from gen3c_b200 import ops
 
     heads, Lq, Lk = 2, 512, 2048

@@ -11,20 +11,20 @@ stored in bf16 sits at 7e-3 (one block) ... 3e-2 (28 blocks) from its own fp32 r
 reachable by any bf16-operand implementation, the reference included.  The bar asserted here is therefore
     err(engine vs fp32) <= err(bf16 run of the reference graph vs fp32)    at every depth,
 i.e. the engine is at least as close to the exact result as the reference's own precision, plus an absolute cap that
-catches gross errors.  The measured numbers are in profiles/r02_parity.txt."""
+catches gross errors."""
 import os
 
 import numpy as np
 import pytest
 import torch
 
-from oracle import cases, dit_oracle, parity
+from oracle import cases, dit_oracle, golden, parity
 
 pytestmark = pytest.mark.gpu
 
 
 def test_fullwidth_block_matches_reference_golden(golden_dir):
-    g = np.load(os.path.join(golden_dir, "dit_fullwidth.npz"))
+    g = golden.load(golden_dir, "dit_fullwidth")
     cfg, shp = cases.FULLWIDTH_1BLOCK, cases.FULLWIDTH_SHAPE
     sd = dit_oracle.random_state_dict(cfg, seed=21)      # the CPU generator: same numbers as when the golden was minted
     net = parity.build_engine_net(cfg, sd, 1, "cuda")
@@ -45,7 +45,7 @@ def test_7b_28_blocks_7040_tokens_matches_fp32_oracle():
 
 @pytest.mark.timeout(900)
 def test_7b_28_blocks_full_56320_tokens_matches_fp32_oracle():
-    """The BASELINE workload itself: latent [16,16,88,160], 28 blocks; the engine takes the CTA-pair GEMM and the
-    cluster-multicast attention paths exactly as in bench.py.  The fp32 oracle costs ~2.2e15 fp32 FLOP on the GPU."""
+    """The BASELINE workload itself: latent [16,16,88,160], 28 blocks; the engine takes the same GEMM and attention
+    paths as bench.py.  The fp32 oracle costs ~2.2e15 fp32 FLOP on the GPU."""
     res = parity.depth_sweep(T=16, depths=(28,), with_bf16=False)
     assert res[28]["engine"] < 3e-2, res

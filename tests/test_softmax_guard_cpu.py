@@ -1,8 +1,10 @@
-"""CPU model of the attention kernel's default softmax (gen3c_b200/csrc/attn_tcgen05.cu, kMode 2): exact row max for the
-first 128-key tile only, stale reference afterwards, reference shifted by a tile's row-sum exponent when it exceeds 2^40,
-sticky overflow flag -> exact second pass.  The model follows the kernel step by step in float32 (P rounded to bf16 for
-the P.V product, as the TMEM A operand is) and must agree with an fp64 softmax on benign, drifting and adversarial score
-distributions — the same cases the GPU tests run through the C ABI (tests/test_dit_ops_gpu.py)."""
+"""CPU model of the sum-guarded online softmax, the cheaper alternative to an exact row max per KV tile: exact row max for
+the first 128-key tile only, stale reference afterwards, reference shifted by a tile's row-sum exponent when it exceeds
+2^40, sticky overflow flag -> exact second pass.  The model runs step by step in float32 (P rounded to bf16 for the P.V
+product, as a bf16 MMA operand is) and must agree with an fp64 softmax on benign, drifting and adversarial score
+distributions — the same cases the GPU tests run through the C ABI (tests/test_dit_ops_gpu.py).  The attention kernel
+(gen3c_b200/csrc/attn_wgmma.cu) uses the exact per-tile row max, i.e. the `exact=True` sweep of this model; the guarded
+sweep is kept validated here as the candidate for removing the per-tile max reduction."""
 import numpy as np
 import pytest
 import torch

@@ -7,14 +7,14 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import cases
+from oracle import cases, golden
 
 
 @pytest.mark.parametrize("tag,bf16", [("f32", False), ("bf16", True)])
 def test_video_jit_tokenizer_matches_reference(tmp_path, golden_dir, tag, bf16):
     from gen3c_b200.pretrained_vae import VideoJITTokenizer
 
-    g = np.load(os.path.join(golden_dir, "vae_wrapper.npz"))
+    g = golden.load(golden_dir, "vae_wrapper")
     cases.write_tiny_tokenizer(str(tmp_path))
     tok = VideoJITTokenizer(name="tiny", latent_ch=16, is_bf16=bf16, spatial_compression_factor=8,
                             temporal_compression_factor=8, pixel_chunk_duration=17, max_enc_batch_size=1,

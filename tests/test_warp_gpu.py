@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import cases, warp_oracle
+from oracle import cases, golden, warp_oracle
 
 pytestmark = pytest.mark.gpu
 
@@ -24,7 +24,7 @@ def close_frac(a, b, atol):
 def test_forward_warp_matches_reference_golden(name, golden_dir):
     from gen3c_b200 import warp
 
-    g = np.load(os.path.join(golden_dir, f"warp_{name}.npz"))
+    g = golden.load(golden_dir, f"warp_{name}")
     c = cases.warp_case(name)
     pts = warp.unproject_points(cu(c["depth"]), cu(c["w2c_src"]), cu(c["K"]))
     np.testing.assert_allclose(pts.cpu().numpy(), g["points"], atol=5e-5, rtol=1e-5)
@@ -48,7 +48,7 @@ def test_splat_indices_bit_exact(name, golden_dir):
     """Integer work: floor/ceil/clamp destination indices on the reference's own coordinates."""
     from gen3c_b200 import warp
 
-    g = np.load(os.path.join(golden_dir, f"warp_{name}.npz"))
+    g = golden.load(golden_dir, f"warp_{name}")
     idx = warp.splat_indices(cu(g["flow"])).cpu().numpy()
     assert np.array_equal(idx[:, 0], g["floor"][:, 0]) and np.array_equal(idx[:, 1], g["floor"][:, 1])
     assert np.array_equal(idx[:, 2], g["ceil"][:, 0]) and np.array_equal(idx[:, 3], g["ceil"][:, 1])
@@ -58,7 +58,7 @@ def test_bilinear_splatting_on_shared_coordinates(golden_dir):
     """Splat alone on the reference's flow/depth: only atomics order and exp/log ulps differ."""
     from gen3c_b200 import warp
 
-    g = np.load(os.path.join(golden_dir, "warp_R6.npz"))
+    g = golden.load(golden_dir, "warp_R6")
     c = cases.warp_case("R6")
     z = warp_oracle.project_points(g["points"], c["w2c_tgt"], c["K"])[:, :, :, 2][:, None]
     mask = (z > 0).astype(np.float32)
@@ -84,7 +84,7 @@ def test_render_cache_matches_reference_golden(golden_dir):
     """Cache3D render, N=2 buffers, F=3 targets, chunk-of-2 max coupling (cache_3d.py:175-223)."""
     from gen3c_b200 import warp
 
-    g = np.load(os.path.join(golden_dir, "warp_cache.npz"))
+    g = golden.load(golden_dir, "warp_cache")
     c = cases.warp_case("R3")
     F = 3
     w2cs = cases.pan_trajectory(F, 0.1)[None]
@@ -131,7 +131,7 @@ def test_foreground_masking_matches_reference_golden(golden_dir):
     (mesh depth within float round-off of `splatted depth - 0.02`)."""
     from gen3c_b200 import warp
 
-    g = np.load(os.path.join(golden_dir, "warp_R7_foreground.npz"))
+    g = golden.load(golden_dir, "warp_R7_foreground")
     c = cases.foreground_case()
     w, m, d, _ = warp.forward_warp(cu(c["image"]), None, None, None, cu(c["w2c_tgt"]), cu(c["K"]), cu(c["K"]),
                                    world_points1=cu(g["points"]), foreground_masking=True, boundary_mask=cu(g["boundary"]))
