@@ -10,13 +10,20 @@
 //                                             all-gather, 1 otherwise)
 //   O  [Lq, heads*128]
 //
-// One CTA = 128 query rows of one head, 384 threads (three warpgroups):
-//   warpgroup 0     TMA producer: Q once, then K_j / V^T_j through a ring of ATT_STAGES 64 KB stages (separate
-//                   barriers for K and V, so S = Q K^T of a step starts before its V has landed)
-//   warpgroups 1-2  consumers, 64 query rows each:  S = Q K_j^T (wgmma, A and B from shared memory) -> online
-//                   softmax in registers (exact row max per 128-key tile, rescale of O) -> P converted in
-//                   place to the bf16 A fragments of O += P V_j (wgmma with A from registers).
-// The two consumer warpgroups run the same step independently, so the softmax of one overlaps the MMAs of the other.
+// One CTA = ATT_ROWS_PER_CTA (128) query rows of one head, 384 threads (three warpgroups):
+//   warpgroup 0     TMA producer: Q once, then K_j and V^T_j through two rings of ATT_STAGES 32 KB stages each (a K
+//                   ring and a V ring with their own full / empty barriers: step j of a consumer reads K_j and V_{j-1})
+//   warpgroups 1-2  consumers, 64 query rows each, software-pipelined with one S tile of lookahead:
+//                     prologue  S_0 = Q K_0^T, softmax, pack P_0
+//                     step j    [turn] issue S_j = Q K_j^T and O += P_{j-1} V_{j-1} [pass turn]; wait<1> (S_j done,
+//                               release K_j); row max and 2^(s - m) of S_j in place; wait<0> (P.V done, release
+//                               V_{j-1}); rescale O and l; pack P_j (bf16 A fragments of the next P.V, from registers)
+//                     epilogue  [turn] O += P_{n-1} V_{n-1} [pass turn]; wait<0>; normalise and store
+//                   so the softmax of step j runs under this warpgroup's own P.V(j-1).  Between the two warpgroups a turn
+//                   token (two mbarriers) alternates the MMA issue, so one warpgroup's softmax sits under the other's
+//                   MMAs instead of both drifting into the softmax together.  Both warpgroups take n_kv + 1 turns,
+//                   including one whose rows are all past Lq (it masks at the store).
+// The protocol (rings, wgmma group waits, turn token) is modelled in tests/test_attn_pingpong_model_cpu.py.
 #include <cmath>
 #include <cstdlib>
 
@@ -25,11 +32,15 @@
 namespace g3c {
 
 constexpr int ATT_THREADS = 384;
-constexpr int ATT_TILE = 128;              // query rows per CTA, keys per KV tile, head dim
-constexpr int ATT_HALF_BYTES = 128 * 128;  // one 64-column half of a 128x128 bf16 tile
+constexpr int ATT_TILE = ATT_ROWS_PER_CTA;  // query rows per CTA, keys per KV tile, head dim
+constexpr int ATT_HALF_BYTES = 128 * 128;   // one 64-column half of a 128x128 bf16 tile
 constexpr int ATT_TILE_BYTES = 2 * ATT_HALF_BYTES;
+// Depth of each of the K and V rings.  3 stages (224 KB with Q) also fit, but measured slower on an H100 SXM at 700 W
+// (sustained 56 320 x 56 320 x 32 heads: 604 TFLOP/s against 613 with 2 stages).
 constexpr int ATT_STAGES = 2;
 constexpr int ATT_SMEM = ATT_TILE_BYTES + ATT_STAGES * 2 * ATT_TILE_BYTES + 256 + 1024;
+static_assert(ATT_SMEM <= 227 * 1024, "attention: Q + K/V rings exceed the 227 KB of shared memory per block");
+static_assert(1 + 4 * ATT_STAGES + 3 <= 256 / 8, "attention: barriers exceed their 256-byte area");
 
 struct AttnParams {
   int Lq, Lk, heads;
@@ -43,7 +54,8 @@ struct AttnParams {
   unsigned long long peer_timeout_ns;  // bound of the wait for a peer's chunk flag (and of this CTA's barrier waits
                                        // while such a wait may be pending): an inter-process dependency, not a protocol bug
   unsigned long long* wait_ns;         // optional profiling counter: ns spent polling chunk flags, summed over CTAs
-  unsigned long long* trace;           // kTrace only: [3 roles][64 steps][8 slots] clock64 stamps of CTA (0,0)
+  unsigned long long* trace;           // kTrace only: [3 roles][64 steps][8 slots] clock64 stamps of CTA (0,0), see
+                                       // g3c_attn_set_trace in include/gen3c_b200.h
 };
 
 static unsigned long long* g_attn_trace = nullptr;
@@ -62,6 +74,66 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return y;
 }
 
+// Online softmax of one S tile (this thread's two rows): exact row max of the tile, new running max m, correction
+// alpha = 2^(m_old - m_new), and S <- 2^(S sl2 - m_new) in place with the row sums l <- l alpha + sum.
+__device__ __forceinline__ void softmax_tile(float (&s)[64], float (&m_run)[2], float (&l_run)[2], float (&alpha)[2],
+                                             float sl2) {
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    mx[0] = fmaxf(mx[0], fmaxf(s[4 * i], s[4 * i + 1]));
+    mx[1] = fmaxf(mx[1], fmaxf(s[4 * i + 2], s[4 * i + 3]));
+  }
+  float nm[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+    mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+    nm[h] = fmaxf(m_run[h], mx[h] * sl2);
+    alpha[h] = ex2_approx(m_run[h] - nm[h]);  // 0 on the first tile (m_run = -inf)
+    m_run[h] = nm[h];
+    l_run[h] *= alpha[h];
+  }
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    s[4 * i] = ex2_approx(fmaf(s[4 * i], sl2, -nm[0]));
+    s[4 * i + 1] = ex2_approx(fmaf(s[4 * i + 1], sl2, -nm[0]));
+    s[4 * i + 2] = ex2_approx(fmaf(s[4 * i + 2], sl2, -nm[1]));
+    s[4 * i + 3] = ex2_approx(fmaf(s[4 * i + 3], sl2, -nm[1]));
+    l_run[0] += s[4 * i] + s[4 * i + 1];
+    l_run[1] += s[4 * i + 2] + s[4 * i + 3];
+  }
+}
+
+// S = Q K^T of one KV tile: 8 k-steps over the head dimension, A (Q rows of this warpgroup) and B (K tile) in shared memory
+__device__ __forceinline__ void issue_s(float (&s)[64], uint64_t dq, const uint8_t* k_tile) {
+  const uint64_t dk = make_sdesc_sw128(smem_u32(k_tile));
+#pragma unroll
+  for (int kk = 0; kk < 8; ++kk) {  // head dimensions 16 kk .. 16 kk + 15
+    const uint32_t off = (kk >> 2) * ATT_HALF_BYTES + (kk & 3) * 32;
+    wgmma_ss_n128(s, sdesc_advance(dq, off), sdesc_advance(dk, off), kk > 0 ? 1u : 0u);
+  }
+}
+
+// O += P V of one KV tile: P from registers (bf16 A fragments), V^T tile in shared memory
+__device__ __forceinline__ void issue_pv(float (&o)[64], const uint32_t (&pa)[32], const uint8_t* v_tile) {
+  const uint64_t dv = make_sdesc_sw128(smem_u32(v_tile));
+#pragma unroll
+  for (int kk = 0; kk < 8; ++kk) {  // keys 16 kk .. 16 kk + 15 = accumulator columns of S
+    const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
+    wgmma_rs_n128(o, a, sdesc_advance(dv, (kk >> 2) * ATT_HALF_BYTES + (kk & 3) * 32));
+  }
+}
+
+// P as bf16 pairs from the exponentiated S: pa[2i] = row a, pa[2i + 1] = row a + 8, keys 8i + 2 (lane % 4) + {0, 1}
+__device__ __forceinline__ void pack_p(uint32_t (&pa)[32], const float (&s)[64]) {
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    pa[2 * i] = pack_bf16x2(s[4 * i], s[4 * i + 1]);
+    pa[2 * i + 1] = pack_bf16x2(s[4 * i + 2], s[4 * i + 3]);
+  }
+}
+
 template <bool kTrace>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
     k_attn_fwd(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
@@ -73,10 +145,13 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
   uint8_t* smem_k = smem + ATT_TILE_BYTES;                          // [ATT_STAGES] K tiles
   uint8_t* smem_v = smem_k + ATT_STAGES * ATT_TILE_BYTES;            // [ATT_STAGES] V^T tiles
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_v + ATT_STAGES * ATT_TILE_BYTES);
-  uint64_t* q_full = bars;                        // [1]
-  uint64_t* k_full = bars + 1;                    // [ATT_STAGES]
-  uint64_t* v_full = bars + 1 + ATT_STAGES;       // [ATT_STAGES]
-  uint64_t* kv_empty = bars + 1 + 2 * ATT_STAGES; // [ATT_STAGES]
+  uint64_t* q_full = bars;                   // [1]
+  uint64_t* k_full = bars + 1;               // [ATT_STAGES]
+  uint64_t* v_full = k_full + ATT_STAGES;    // [ATT_STAGES]
+  uint64_t* k_empty = v_full + ATT_STAGES;   // [ATT_STAGES]
+  uint64_t* v_empty = k_empty + ATT_STAGES;  // [ATT_STAGES]
+  uint64_t* turn = v_empty + ATT_STAGES;     // [2]: phase t of turn[c] completes when consumer c may take its turn t
+  uint64_t* done = turn + 2;                 // [1]: both consumer warpgroups finished (their waits exit, not trap)
 
   const uint32_t wg = threadIdx.x / 128;
   const uint32_t tid = threadIdx.x % 128;
@@ -92,8 +167,12 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
     for (int i = 0; i < ATT_STAGES; ++i) {
       mbar_init(&k_full[i], 1);
       mbar_init(&v_full[i], 1);
-      mbar_init(&kv_empty[i], 2);  // one arrive per consumer warpgroup
+      mbar_init(&k_empty[i], 2);  // one arrive per consumer warpgroup
+      mbar_init(&v_empty[i], 2);
     }
+    for (int c = 0; c < 2; ++c) mbar_init(&turn[c], 4);  // one arrive per warp of the other consumer warpgroup
+    for (int w = 0; w < 4; ++w) mbar_arrive(&turn[0]);   // consumer 0 holds the first turn
+    mbar_init(done, 2);
     fence_barrier_init();
   }
   __syncthreads();
@@ -126,11 +205,12 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
           asm volatile("fence.proxy.async.global;\n" ::: "memory");  // peer-written data is read by the TMA next
         }
         const int kv0 = chunk * p.vt_chunk_len + within * ATT_TILE;
-        mbar_wait_ns(&kv_empty[stage], phase ^ 1, p.peer_timeout_ns);
+        mbar_wait_ns(&k_empty[stage], phase ^ 1, p.peer_timeout_ns);
         mbar_expect_tx(&k_full[stage], ATT_TILE_BYTES);
         for (int h = 0; h < 2; ++h)  // the two 64-dim halves of 128 keys
           tma_load_2d(smem_k + stage * ATT_TILE_BYTES + h * ATT_HALF_BYTES, &tmK, &k_full[stage], head * 128 + h * 64,
                       kv0);
+        mbar_wait_ns(&v_empty[stage], phase ^ 1, p.peer_timeout_ns);
         mbar_expect_tx(&v_full[stage], ATT_TILE_BYTES);
         for (int h = 0; h < 2; ++h)  // the two 64-key halves of 128 head dimensions
           tma_load_3d(smem_v + stage * ATT_TILE_BYTES + h * ATT_HALF_BYTES, &tmV, &v_full[stage],
@@ -140,68 +220,78 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
           phase ^= 1;
         }
       }
+      // a consumer whose barrier wait timed out has exited without arriving: trap here, within the bound
+      mbar_wait_ns(done, 0, p.peer_timeout_ns);
     }
   } else {
     // ===== consumers: warpgroup c owns query rows [64c, 64c + 64) of the tile =====
     setmaxnreg_inc<240>();
     const uint32_t c = wg - 1;
     const uint32_t warp = tid / 32, lane = tid % 32;
+    const unsigned long long tmo = p.peer_timeout_ns;
     // accumulator layout (wgmma m64n128k16, f32), i in [0, 16): acc[4i + {0,1}] = row 16 warp + lane/4, columns 8i + 2 (lane%4) + {0,1};
     // acc[4i + {2,3}] = the same columns eight rows further down
     float o[64];
 #pragma unroll
     for (int i = 0; i < 64; ++i) o[i] = 0.f;
+    float s[64];      // S_j, then 2^(S_j - m) in place
+    uint32_t pa[32];  // P_{j-1}: the A operand of the P.V in flight during the softmax of step j
     float m_run[2] = {-INFINITY, -INFINITY};  // running row max (log2 units) of the two rows of this thread
     float l_run[2] = {0.f, 0.f};              // this thread's partial row sums (quad-reduced at the end)
+    float alpha[2];
     const float sl2 = p.scale_log2;
     const uint64_t dq = make_sdesc_sw128(smem_u32(smem_q + c * 64 * 128));
-    mbar_wait_ns(q_full, 0, p.peer_timeout_ns);
-    uint32_t stage = 0, phase = 0;
-    for (int j = 0; j < n_kv; ++j) {
+    uint32_t tph = 0;         // parity of this warpgroup's next turn (turn t waits for phase t of turn[c])
+    uint32_t ks = 0, kp = 0;  // ring stage / parity of K_j
+    uint32_t vs = 0, vp = 0;  // ring stage / parity of V_{j-1}
+    int j = 0;
+    // ---- prologue: S_0, softmax, P_0 ----
+    mbar_wait_ns_or_exit(q_full, 0, tmo);
+    mbar_wait_ns_or_exit(&k_full[ks], kp, tmo);
+    mbar_wait_ns_or_exit(&turn[c], tph, tmo);
+    tph ^= 1;
+    ATT_TR(1 + c, 0);
+    wgmma_fence();
+    issue_s(s, dq, smem_k + ks * ATT_TILE_BYTES);
+    wgmma_commit();
+    if (lane == 0) mbar_arrive(&turn[c ^ 1]);
+    ATT_TR(1 + c, 1);
+    wgmma_wait<0>();
+    fence_regs(s);
+    if (tid == 0) mbar_arrive(&k_empty[ks]);
+    ATT_TR(1 + c, 2);
+    softmax_tile(s, m_run, l_run, alpha, sl2);
+    pack_p(pa, s);
+    ATT_TR(1 + c, 3);
+    if (++ks == ATT_STAGES) {
+      ks = 0;
+      kp ^= 1;
+    }
+    // ---- steady state: S_j is computed while P.V(j-1) runs; the softmax of S_j runs under P.V(j-1) ----
+    for (j = 1; j < n_kv; ++j) {
+      mbar_wait_ns_or_exit(&k_full[ks], kp, tmo);
+      mbar_wait_ns_or_exit(&v_full[vs], vp, tmo);
+      mbar_wait_ns_or_exit(&turn[c], tph, tmo);
+      tph ^= 1;
       ATT_TR(1 + c, 0);
-      float s[64];
-      mbar_wait_ns(&k_full[stage], phase, p.peer_timeout_ns);
+      wgmma_fence();
+      issue_s(s, dq, smem_k + ks * ATT_TILE_BYTES);
+      wgmma_commit();
+      issue_pv(o, pa, smem_v + vs * ATT_TILE_BYTES);
+      wgmma_commit();
+      if (lane == 0) mbar_arrive(&turn[c ^ 1]);
       ATT_TR(1 + c, 1);
-      {
-        const uint64_t dk = make_sdesc_sw128(smem_u32(smem_k + stage * ATT_TILE_BYTES));
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {  // head dimensions 16 kk .. 16 kk + 15
-          const uint32_t off = (kk >> 2) * ATT_HALF_BYTES + (kk & 3) * 32;
-          wgmma_ss_n128(s, sdesc_advance(dq, off), sdesc_advance(dk, off), kk > 0 ? 1u : 0u);
-        }
-        wgmma_commit();
-        wgmma_wait<0>();
-        fence_regs(s);
-      }
+      wgmma_wait<1>();  // S_j complete; P.V(j-1) may still run
+      fence_regs(s);
+      if (tid == 0) mbar_arrive(&k_empty[ks]);
       ATT_TR(1 + c, 2);
-      // ---- online softmax (exact row max of every tile) ----
-      float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        mx[0] = fmaxf(mx[0], fmaxf(s[4 * i], s[4 * i + 1]));
-        mx[1] = fmaxf(mx[1], fmaxf(s[4 * i + 2], s[4 * i + 3]));
-      }
-      float alpha[2], nm[2];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
-        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
-        nm[h] = fmaxf(m_run[h], mx[h] * sl2);
-        alpha[h] = ex2_approx(m_run[h] - nm[h]);  // 0 on the first tile (m_run = -inf)
-        m_run[h] = nm[h];
-        l_run[h] *= alpha[h];
-      }
-      uint32_t pa[32];  // P as bf16 pairs: the A fragments of the 8 k-steps of P V
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const float p0 = ex2_approx(fmaf(s[4 * i], sl2, -nm[0])), p1 = ex2_approx(fmaf(s[4 * i + 1], sl2, -nm[0]));
-        const float p2 = ex2_approx(fmaf(s[4 * i + 2], sl2, -nm[1])), p3 = ex2_approx(fmaf(s[4 * i + 3], sl2, -nm[1]));
-        l_run[0] += p0 + p1;
-        l_run[1] += p2 + p3;
-        pa[2 * i] = pack_bf16x2(p0, p1);
-        pa[2 * i + 1] = pack_bf16x2(p2, p3);
-      }
+      softmax_tile(s, m_run, l_run, alpha, sl2);  // P_{j-1} (pa) and O are still read / written by the P.V in flight
+      ATT_TR(1 + c, 3);
+      wgmma_wait<0>();
+      fence_regs(o);
+      fence_regs(pa);  // pa stays allocated (not reused for the exponentials above) until the P.V has read it
+      if (tid == 0) mbar_arrive(&v_empty[vs]);
+      ATT_TR(1 + c, 4);
 #pragma unroll
       for (int i = 0; i < 16; ++i) {
         o[4 * i] *= alpha[0];
@@ -209,28 +299,30 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
         o[4 * i + 2] *= alpha[1];
         o[4 * i + 3] *= alpha[1];
       }
-      ATT_TR(1 + c, 3);
-      // ---- O += P V_j ----
-      mbar_wait_ns(&v_full[stage], phase, p.peer_timeout_ns);
-      {
-        const uint64_t dv = make_sdesc_sw128(smem_u32(smem_v + stage * ATT_TILE_BYTES));
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {  // keys 16 kk .. 16 kk + 15 = accumulator columns of S
-          const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
-          wgmma_rs_n128(o, a, sdesc_advance(dv, (kk >> 2) * ATT_HALF_BYTES + (kk & 3) * 32));
-        }
-        wgmma_commit();
-        wgmma_wait<0>();
-        fence_regs(o);
+      pack_p(pa, s);
+      if (++ks == ATT_STAGES) {
+        ks = 0;
+        kp ^= 1;
       }
-      if (tid == 0) mbar_arrive(&kv_empty[stage]);
-      ATT_TR(1 + c, 4);
-      if (++stage == ATT_STAGES) {
-        stage = 0;
-        phase ^= 1;
+      if (++vs == ATT_STAGES) {
+        vs = 0;
+        vp ^= 1;
       }
     }
+    // ---- epilogue: O += P_{n-1} V_{n-1} (the last turn: both warpgroups take n_kv + 1 turns) ----
+    mbar_wait_ns_or_exit(&v_full[vs], vp, tmo);
+    mbar_wait_ns_or_exit(&turn[c], tph, tmo);
+    ATT_TR(1 + c, 0);
+    wgmma_fence();
+    issue_pv(o, pa, smem_v + vs * ATT_TILE_BYTES);
+    wgmma_commit();
+    if (lane == 0) mbar_arrive(&turn[c ^ 1]);
+    ATT_TR(1 + c, 1);
+    wgmma_wait<0>();
+    fence_regs(o);
+    fence_regs(pa);
+    if (tid == 0) mbar_arrive(&v_empty[vs]);
+    ATT_TR(1 + c, 4);
     // ---- normalise and store ----
     float inv[2];
 #pragma unroll
@@ -250,6 +342,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
       for (int i = 0; i < 16; ++i)
         *reinterpret_cast<uint32_t*>(dst + 8 * i) = pack_bf16x2(o[4 * i + 2 * h] * inv[h], o[4 * i + 2 * h + 1] * inv[h]);
     }
+    if (tid == 0) mbar_arrive(done);
   }
 }
 

@@ -169,6 +169,23 @@ __device__ __forceinline__ void mbar_wait_ns(uint64_t* bar, uint32_t parity, uns
   }
 }
 
+// Same bound, but on timeout the thread exits instead of trapping.  For warpgroups that raised their budget with
+// setmaxnreg.inc: a trap anywhere in such a region makes ptxas allocate it for a smaller budget (the attention consumers
+// then spill and serialise their wgmma).  The kernel still traps: a thread outside the region waits (mbar_wait_ns) on a
+// barrier that these threads only arrive on when they finish normally.
+__device__ __forceinline__ void mbar_wait_ns_or_exit(uint64_t* bar, uint32_t parity, unsigned long long timeout_ns) {
+  if (mbar_try_wait(bar, parity)) return;
+  uint32_t spins = 0;
+  uint64_t t0 = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if ((++spins & 0xFFFu) == 0) {
+      uint64_t now = global_timer_ns();
+      if (t0 == 0) t0 = now;
+      else if (now - t0 > timeout_ns) asm volatile("exit;\n");
+    }
+  }
+}
+
 // ----------------------------------------------------------------------------------------------
 // TMA loads (tile mode, mbarrier completion)
 // ----------------------------------------------------------------------------------------------
@@ -231,6 +248,12 @@ template <int N>
 __device__ __forceinline__ void fence_regs(float (&r)[N]) {
 #pragma unroll
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
+// Same for the register A fragments of a wgmma still in flight: keeps them live (their registers are not reused) until here.
+template <int N>
+__device__ __forceinline__ void fence_regs(uint32_t (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(r[i])::"memory");
 }
 
 // Shared-memory matrix descriptor of a K-major tile stored with the 128-byte swizzle (rows of 64 bf16 = 128 B, 8-row

@@ -481,7 +481,7 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
         gate.seq = seq;
         gate.first = me;
         gate.wait_ns = h->prof ? h->wait_ns : nullptr;
-        h->wait_cta_launches = (double)((L + 255) / 256) * heads;  // CTAs of one gated launch
+        h->wait_cta_launches = (double)((L + ATT_ROWS_PER_CTA - 1) / ATT_ROWS_PER_CTA) * heads;  // CTAs of one gated launch
         K(CAT_ATTN_SELF, attn_fwd(h->q, kb, vb, h->att, L, Lk_all, heads, D, D, D, L, attn_scale, st, &gate));
       } else {
         TRY(proj_norm_rope(h->xn, s.wk, k_loc, L, D, s.gk, h->rope, n));

@@ -32,6 +32,8 @@ struct ChunkGate {
   unsigned long long* wait_ns = nullptr;  // optional: += ns each CTA's loader spent polling flags (profiling)
 };
 unsigned long long peer_timeout_ns();  // bound of inter-process waits (G3C_PEER_TIMEOUT_S, default 600 s)
+// attn_fwd launches one CTA per ATT_ROWS_PER_CTA query rows of one head (also its KV tile width: Lk % 128 == 0)
+constexpr int ATT_ROWS_PER_CTA = 128;
 int attn_fwd(const void* q, const void* k, const void* vt, void* o, int Lq, int Lk, int heads,
              int ldq, int ldk, int ldo, int vt_chunk_len, float scale, cudaStream_t st,
              const ChunkGate* gate = nullptr);

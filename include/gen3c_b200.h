@@ -144,9 +144,10 @@ int g3c_attn_fwd(const void* q, const void* k, const void* vt, void* o, int Lq, 
                  int ldq, int ldk, int ldo, int vt_chunk_len, float scale, void* stream);
 
 /* Profiling aid: when a device buffer of 3*64*8 uint64 is registered, the next g3c_attn_fwd launches run a
- * traced build of the kernel in which CTA (0,0) records clock64() stamps per KV step (first 64 steps): roles 1/2 = the
- * two consumer warpgroups; slots 0 step start, 1 K landed, 2 S = Q K^T done, 3 softmax done, 4 P V done.  NULL
- * switches tracing off. */
+ * traced build of the kernel in which CTA (0,0) records clock64() stamps per KV step j (first 64 steps): roles 1/2 =
+ * the two consumer warpgroups; slots 0 turn acquired, 1 MMAs of the step issued (S_j and P_{j-1} V_{j-1}), 2 S_j
+ * complete, 3 softmax of S_j done, 4 P_{j-1} V_{j-1} complete.  Step 0 has no P.V; step n_kv (the last P.V) stamps
+ * slots 0, 1 and 4 only.  NULL switches tracing off. */
 int g3c_attn_set_trace(unsigned long long* device_buffer);
 
 /* x (f32 [L,D]) += pos (bf16, optional) ; y (bf16) = LayerNorm_eps(x) * (1 + scale) + shift
