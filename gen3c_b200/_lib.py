@@ -84,6 +84,7 @@ SIGNATURES = {
     "g3c_gemm_bf16": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _I, _P]),
     "g3c_gemm_norm_rope_bf16": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _F, _P]),
     "g3c_attn_fwd": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _F, _P]),
+    "g3c_attn_fwd_sbhd": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _F, _P]),
     "g3c_attn_set_trace": (_I, [_P]),
     "g3c_ln_modulate": (_I, [_P, _P, _P, _P, _P, _I, _I, _F, _P]),
     "g3c_rmsnorm_rope": (_I, [_P, _I, _I, _I, _P, _P, _F, _P]),

@@ -9,6 +9,7 @@
 //                                             `chunks` = context-parallel ranks after the KV
 //                                             all-gather, 1 otherwise)
 //   O  [Lq, heads*128]
+//   kVTokenMajor (g3c_attn_fwd_sbhd): V [Lk, heads*128] token-major like K, any Lk >= 1, heads = batch x heads of sbhd
 //
 // One CTA = ATT_ROWS_PER_CTA (128) query rows of one head, 384 threads (three warpgroups):
 //   warpgroup 0     TMA producer: Q once, then K_j and V^T_j through two rings of ATT_STAGES 32 KB stages each (a K
@@ -115,13 +116,37 @@ __device__ __forceinline__ void issue_s(float (&s)[64], uint64_t dq, const uint8
   }
 }
 
-// O += P V of one KV tile: P from registers (bf16 A fragments), V^T tile in shared memory
+// O += P V of one KV tile: P from registers (bf16 A fragments), V in shared memory.  V^T tile (keys contiguous): K-major
+// B.  Token-major V tile (kVTokenMajor; head dims contiguous, loaded like K): MN-major B whose two 64-dim halves are
+// ATT_HALF_BYTES apart (LBO), and k-step kk starts 16 keys of 128-byte rows into each half.
+template <bool kVTokenMajor>
 __device__ __forceinline__ void issue_pv(float (&o)[64], const uint32_t (&pa)[32], const uint8_t* v_tile) {
-  const uint64_t dv = make_sdesc_sw128(smem_u32(v_tile));
+  if constexpr (kVTokenMajor) {
+    const uint64_t dv = make_sdesc_sw128_mn(smem_u32(v_tile), ATT_HALF_BYTES);
 #pragma unroll
-  for (int kk = 0; kk < 8; ++kk) {  // keys 16 kk .. 16 kk + 15 = accumulator columns of S
-    const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
-    wgmma_rs_n128(o, a, sdesc_advance(dv, (kk >> 2) * ATT_HALF_BYTES + (kk & 3) * 32));
+    for (int kk = 0; kk < 8; ++kk) {
+      const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
+      wgmma_rs_n128_tb(o, a, sdesc_advance(dv, kk * 16 * 128));
+    }
+  } else {
+    const uint64_t dv = make_sdesc_sw128(smem_u32(v_tile));
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {  // keys 16 kk .. 16 kk + 15 = accumulator columns of S
+      const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
+      wgmma_rs_n128(o, a, sdesc_advance(dv, (kk >> 2) * ATT_HALF_BYTES + (kk & 3) * 32));
+    }
+  }
+}
+
+// Last KV tile when Lk % 128 != 0: the TMA zero-filled the K rows past Lk, whose scores (0) would still enter the
+// softmax.  Columns >= `valid` (keys of this tile below Lk, 1..128) are set to -inf before the row max, so their
+// exponentials are 0.
+__device__ __forceinline__ void mask_key_tail(float (&s)[64], int valid, uint32_t lane) {
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    const int col = 8 * i + 2 * (int)(lane % 4);
+    if (col >= valid) s[4 * i] = s[4 * i + 2] = -INFINITY;
+    if (col + 1 >= valid) s[4 * i + 1] = s[4 * i + 3] = -INFINITY;
   }
 }
 
@@ -134,7 +159,9 @@ __device__ __forceinline__ void pack_p(uint32_t (&pa)[32], const float (&s)[64])
   }
 }
 
-template <bool kTrace>
+// kVTokenMajor: V is [Lk, heads*128] like K (instead of the chunked V^T), any Lk >= 1 (the last KV tile is partial and
+// masked), no context-parallel gate.
+template <bool kTrace, bool kVTokenMajor = false>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
     k_attn_fwd(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
@@ -157,7 +184,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
   const uint32_t tid = threadIdx.x % 128;
   const int head = blockIdx.y;
   const int q0 = blockIdx.x * ATT_TILE;
-  const int n_kv = p.Lk / ATT_TILE;
+  const int n_kv = kVTokenMajor ? (p.Lk + ATT_TILE - 1) / ATT_TILE : p.Lk / ATT_TILE;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
@@ -187,22 +214,25 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
       const int n_chunks = p.Lk / p.vt_chunk_len;
       uint32_t stage = 0, phase = 0;
       for (int j = 0; j < n_kv; ++j) {
-        // KV tiles are visited chunk by chunk starting with `first_chunk` (the local one under context
-        // parallelism); a remote chunk is only touched after its producer rank has published it.
-        int chunk = p.first_chunk + j / tiles_per_chunk;
-        if (chunk >= n_chunks) chunk -= n_chunks;
-        const int within = j % tiles_per_chunk;
-        if (p.chunk_flags && within == 0 && chunk != p.first_chunk) {  // the local chunk is ordered by the stream
-          uint32_t v, spins = 0;
-          uint64_t t0 = 0;
-          for (;;) {
-            asm volatile("ld.acquire.sys.global.u32 %0, [%1];\n" : "=r"(v) : "l"(p.chunk_flags + chunk) : "memory");
-            if ((int)(v - p.flag_seq) >= 0) break;
-            if (t0 == 0) t0 = global_timer_ns();
-            if ((++spins & 0x3FFu) == 0 && global_timer_ns() - t0 > p.peer_timeout_ns) asm volatile("trap;\n");
+        int chunk = 0, within = j;  // token-major V: one chunk of all Lk keys
+        if constexpr (!kVTokenMajor) {
+          // KV tiles are visited chunk by chunk starting with `first_chunk` (the local one under context
+          // parallelism); a remote chunk is only touched after its producer rank has published it.
+          chunk = p.first_chunk + j / tiles_per_chunk;
+          if (chunk >= n_chunks) chunk -= n_chunks;
+          within = j % tiles_per_chunk;
+          if (p.chunk_flags && within == 0 && chunk != p.first_chunk) {  // the local chunk is ordered by the stream
+            uint32_t v, spins = 0;
+            uint64_t t0 = 0;
+            for (;;) {
+              asm volatile("ld.acquire.sys.global.u32 %0, [%1];\n" : "=r"(v) : "l"(p.chunk_flags + chunk) : "memory");
+              if ((int)(v - p.flag_seq) >= 0) break;
+              if (t0 == 0) t0 = global_timer_ns();
+              if ((++spins & 0x3FFu) == 0 && global_timer_ns() - t0 > p.peer_timeout_ns) asm volatile("trap;\n");
+            }
+            if (t0 != 0 && p.wait_ns) atomicAdd(p.wait_ns, (unsigned long long)(global_timer_ns() - t0));
+            asm volatile("fence.proxy.async.global;\n" ::: "memory");  // peer-written data is read by the TMA next
           }
-          if (t0 != 0 && p.wait_ns) atomicAdd(p.wait_ns, (unsigned long long)(global_timer_ns() - t0));
-          asm volatile("fence.proxy.async.global;\n" ::: "memory");  // peer-written data is read by the TMA next
         }
         const int kv0 = chunk * p.vt_chunk_len + within * ATT_TILE;
         mbar_wait_ns(&k_empty[stage], phase ^ 1, p.peer_timeout_ns);
@@ -212,9 +242,14 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
                       kv0);
         mbar_wait_ns(&v_empty[stage], phase ^ 1, p.peer_timeout_ns);
         mbar_expect_tx(&v_full[stage], ATT_TILE_BYTES);
-        for (int h = 0; h < 2; ++h)  // the two 64-key halves of 128 head dimensions
-          tma_load_3d(smem_v + stage * ATT_TILE_BYTES + h * ATT_HALF_BYTES, &tmV, &v_full[stage],
-                      within * ATT_TILE + h * 64, head * 128, chunk);
+        for (int h = 0; h < 2; ++h) {
+          if constexpr (kVTokenMajor)  // as K: the two 64-dim halves of 128 keys
+            tma_load_2d(smem_v + stage * ATT_TILE_BYTES + h * ATT_HALF_BYTES, &tmV, &v_full[stage],
+                        head * 128 + h * 64, kv0);
+          else  // the two 64-key halves of 128 head dimensions
+            tma_load_3d(smem_v + stage * ATT_TILE_BYTES + h * ATT_HALF_BYTES, &tmV, &v_full[stage],
+                        within * ATT_TILE + h * 64, head * 128, chunk);
+        }
         if (++stage == ATT_STAGES) {
           stage = 0;
           phase ^= 1;
@@ -260,6 +295,9 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
     fence_regs(s);
     if (tid == 0) mbar_arrive(&k_empty[ks]);
     ATT_TR(1 + c, 2);
+    if constexpr (kVTokenMajor) {
+      if (n_kv == 1) mask_key_tail(s, p.Lk, lane);
+    }
     softmax_tile(s, m_run, l_run, alpha, sl2);
     pack_p(pa, s);
     ATT_TR(1 + c, 3);
@@ -268,7 +306,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
       kp ^= 1;
     }
     // ---- steady state: S_j is computed while P.V(j-1) runs; the softmax of S_j runs under P.V(j-1) ----
-    for (j = 1; j < n_kv; ++j) {
+    for (j = 1; j < (kVTokenMajor ? n_kv - 1 : n_kv); ++j) {
       mbar_wait_ns_or_exit(&k_full[ks], kp, tmo);
       mbar_wait_ns_or_exit(&v_full[vs], vp, tmo);
       mbar_wait_ns_or_exit(&turn[c], tph, tmo);
@@ -277,7 +315,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
       wgmma_fence();
       issue_s(s, dq, smem_k + ks * ATT_TILE_BYTES);
       wgmma_commit();
-      issue_pv(o, pa, smem_v + vs * ATT_TILE_BYTES);
+      issue_pv<kVTokenMajor>(o, pa, smem_v + vs * ATT_TILE_BYTES);
       wgmma_commit();
       if (lane == 0) mbar_arrive(&turn[c ^ 1]);
       ATT_TR(1 + c, 1);
@@ -309,12 +347,54 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
         vp ^= 1;
       }
     }
+    if constexpr (kVTokenMajor) {
+      // ---- the last KV tile, peeled off the loop: the same step with the keys past Lk masked before the row max ----
+      if (n_kv > 1) {
+        mbar_wait_ns_or_exit(&k_full[ks], kp, tmo);
+        mbar_wait_ns_or_exit(&v_full[vs], vp, tmo);
+        mbar_wait_ns_or_exit(&turn[c], tph, tmo);
+        tph ^= 1;
+        ATT_TR(1 + c, 0);
+        wgmma_fence();
+        issue_s(s, dq, smem_k + ks * ATT_TILE_BYTES);
+        wgmma_commit();
+        issue_pv<kVTokenMajor>(o, pa, smem_v + vs * ATT_TILE_BYTES);
+        wgmma_commit();
+        if (lane == 0) mbar_arrive(&turn[c ^ 1]);
+        ATT_TR(1 + c, 1);
+        wgmma_wait<1>();  // S_j complete; P.V(j-1) may still run
+        fence_regs(s);
+        if (tid == 0) mbar_arrive(&k_empty[ks]);
+        ATT_TR(1 + c, 2);
+        mask_key_tail(s, p.Lk - j * ATT_TILE, lane);
+        softmax_tile(s, m_run, l_run, alpha, sl2);
+        ATT_TR(1 + c, 3);
+        wgmma_wait<0>();
+        fence_regs(o);
+        fence_regs(pa);  // pa stays allocated (not reused for the exponentials above) until the P.V has read it
+        if (tid == 0) mbar_arrive(&v_empty[vs]);
+        ATT_TR(1 + c, 4);
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          o[4 * i] *= alpha[0];
+          o[4 * i + 1] *= alpha[0];
+          o[4 * i + 2] *= alpha[1];
+          o[4 * i + 3] *= alpha[1];
+        }
+        pack_p(pa, s);
+        if (++vs == ATT_STAGES) {
+          vs = 0;
+          vp ^= 1;
+        }
+      }
+      j = n_kv;
+    }
     // ---- epilogue: O += P_{n-1} V_{n-1} (the last turn: both warpgroups take n_kv + 1 turns) ----
     mbar_wait_ns_or_exit(&v_full[vs], vp, tmo);
     mbar_wait_ns_or_exit(&turn[c], tph, tmo);
     ATT_TR(1 + c, 0);
     wgmma_fence();
-    issue_pv(o, pa, smem_v + vs * ATT_TILE_BYTES);
+    issue_pv<kVTokenMajor>(o, pa, smem_v + vs * ATT_TILE_BYTES);
     wgmma_commit();
     if (lane == 0) mbar_arrive(&turn[c ^ 1]);
     ATT_TR(1 + c, 1);
@@ -346,6 +426,19 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
   }
 }
 
+// TMA map of a token-major operand [rows, heads*128] (leading dimension ld): boxes of 64 head dims x 128 tokens
+static int make_tmap_tokens(CUtensorMap* m, const void* base, int rows, int heads, int ld) {
+  uint64_t dims[2] = {(uint64_t)heads * 128, (uint64_t)rows}, str[1] = {(uint64_t)ld * 2};
+  uint32_t box[2] = {64, 128};
+  return make_tmap_bf16_sw128(m, base, 2, dims, str, box);
+}
+
+// scale = ln 2 declares that Q already carries softmax scale * log2(e): S is then in log2 units
+static float scale_log2(float scale) {
+  const float s = scale * 1.4426950408889634f;
+  return fabsf(s - 1.0f) < 1e-6f ? 1.0f : s;
+}
+
 int attn_fwd(const void* q, const void* k, const void* vt, void* o, int Lq, int Lk, int heads,
              int ldq, int ldk, int ldo, int vt_chunk_len, float scale, cudaStream_t st, const ChunkGate* gate) {
   G3C_REQUIRE(q && k && vt && o, "attn: null operand");
@@ -359,24 +452,16 @@ int attn_fwd(const void* q, const void* k, const void* vt, void* o, int Lq, int 
               "attn: leading dimensions must be >= heads*128 and multiples of 8");
   G3C_REQUIRE((reinterpret_cast<uintptr_t>(o) & 15) == 0, "attn: O must be 16-byte aligned");
   CUtensorMap tmQ, tmK, tmV;
-  {
-    uint64_t dims[2] = {(uint64_t)heads * 128, (uint64_t)Lq}, str[1] = {(uint64_t)ldq * 2};
-    uint32_t box[2] = {64, 128};
-    int rc = make_tmap_bf16_sw128(&tmQ, q, 2, dims, str, box);
-    if (rc) return rc;
-  }
-  {
-    uint64_t dims[2] = {(uint64_t)heads * 128, (uint64_t)Lk}, str[1] = {(uint64_t)ldk * 2};
-    uint32_t box[2] = {64, 128};
-    int rc = make_tmap_bf16_sw128(&tmK, k, 2, dims, str, box);
-    if (rc) return rc;
-  }
+  int rc = make_tmap_tokens(&tmQ, q, Lq, heads, ldq);
+  if (rc) return rc;
+  rc = make_tmap_tokens(&tmK, k, Lk, heads, ldk);
+  if (rc) return rc;
   {
     const int chunks = Lk / vt_chunk_len;
     uint64_t dims[3] = {(uint64_t)vt_chunk_len, (uint64_t)heads * 128, (uint64_t)chunks};
     uint64_t str[2] = {(uint64_t)vt_chunk_len * 2, (uint64_t)vt_chunk_len * 2 * heads * 128};
     uint32_t box[3] = {64, 128, 1};
-    int rc = make_tmap_bf16_sw128(&tmV, vt, 3, dims, str, box);
+    rc = make_tmap_bf16_sw128(&tmV, vt, 3, dims, str, box);
     if (rc) return rc;
   }
   static bool configured = false;
@@ -392,9 +477,7 @@ int attn_fwd(const void* q, const void* k, const void* vt, void* o, int Lq, int 
   p.ldo = ldo;
   p.vt_chunk_len = vt_chunk_len;
   p.O = reinterpret_cast<__nv_bfloat16*>(o);
-  // scale = ln 2 declares that Q already carries softmax scale * log2(e): S is then in log2 units
-  p.scale_log2 = scale * 1.4426950408889634f;
-  if (fabsf(p.scale_log2 - 1.0f) < 1e-6f) p.scale_log2 = 1.0f;
+  p.scale_log2 = scale_log2(scale);
   p.chunk_flags = gate ? gate->flags : nullptr;
   p.peer_timeout_ns = gate ? peer_timeout_ns() : G3C_MBAR_TIMEOUT_NS;
   p.wait_ns = gate ? gate->wait_ns : nullptr;
@@ -405,6 +488,49 @@ int attn_fwd(const void* q, const void* k, const void* vt, void* o, int Lq, int 
   dim3 grid((Lq + ATT_TILE - 1) / ATT_TILE, heads);
   if (g_attn_trace) k_attn_fwd<true><<<grid, ATT_THREADS, ATT_SMEM, st>>>(tmQ, tmK, tmV, p);
   else k_attn_fwd<false><<<grid, ATT_THREADS, ATT_SMEM, st>>>(tmQ, tmK, tmV, p);
+  G3C_CUDA(cudaGetLastError());
+  return G3C_OK;
+}
+
+// q, k, v, o: `batch` x `heads` heads of 128 per token (the rows of contiguous sbhd [s, b, h, 128] tensors viewed as
+// [s, b*h*128]), so the batch is b*h heads of one launch.  V token-major like K; any Lq, Lk >= 1.
+int attn_fwd_sbhd(const void* q, const void* k, const void* v, void* o, int Lq, int Lk, int batch, int heads, int ldq,
+                  int ldk, int ldv, int ldo, float scale, cudaStream_t st) {
+  G3C_REQUIRE(q && k && v && o, "attn_sbhd: null operand");
+  G3C_REQUIRE(Lq > 0 && Lk > 0, "attn_sbhd: Lq=%d and Lk=%d must be >= 1", Lq, Lk);
+  G3C_REQUIRE(batch > 0 && heads > 0 && (long long)batch * heads <= 65535,
+              "attn_sbhd: batch=%d x heads=%d must be in [1, 65535]", batch, heads);
+  const int bh = batch * heads;
+  G3C_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0 && ldq >= bh * 128 && ldk >= bh * 128 &&
+                  ldv >= bh * 128 && ldo >= bh * 128,
+              "attn_sbhd: leading dimensions (%d, %d, %d, %d) must be >= batch*heads*128 = %d and multiples of 8", ldq,
+              ldk, ldv, ldo, bh * 128);
+  G3C_REQUIRE(((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
+                reinterpret_cast<uintptr_t>(o)) & 15) == 0,
+              "attn_sbhd: q, k, v and o must be 16-byte aligned");
+  CUtensorMap tmQ, tmK, tmV;
+  int rc = make_tmap_tokens(&tmQ, q, Lq, bh, ldq);
+  if (rc) return rc;
+  rc = make_tmap_tokens(&tmK, k, Lk, bh, ldk);
+  if (rc) return rc;
+  rc = make_tmap_tokens(&tmV, v, Lk, bh, ldv);
+  if (rc) return rc;
+  static bool configured = false;
+  if (!configured) {
+    G3C_CUDA(cudaFuncSetAttribute(k_attn_fwd<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
+    configured = true;
+  }
+  AttnParams p = {};
+  p.Lq = Lq;
+  p.Lk = Lk;
+  p.heads = bh;
+  p.ldo = ldo;
+  p.vt_chunk_len = Lk;
+  p.O = reinterpret_cast<__nv_bfloat16*>(o);
+  p.scale_log2 = scale_log2(scale);
+  p.peer_timeout_ns = G3C_MBAR_TIMEOUT_NS;
+  dim3 grid((Lq + ATT_TILE - 1) / ATT_TILE, bh);
+  k_attn_fwd<false, true><<<grid, ATT_THREADS, ATT_SMEM, st>>>(tmQ, tmK, tmV, p);
   G3C_CUDA(cudaGetLastError());
   return G3C_OK;
 }
@@ -421,4 +547,9 @@ extern "C" int g3c_attn_fwd(const void* q, const void* k, const void* vt, void* 
                             void* stream) {
   return g3c::attn_fwd(q, k, vt, o, Lq, Lk, heads, ldq, ldk, ldo, vt_chunk_len, scale,
                        (cudaStream_t)stream, nullptr);
+}
+
+extern "C" int g3c_attn_fwd_sbhd(const void* q, const void* k, const void* v, void* o, int Lq, int Lk, int batch,
+                                 int heads, int ldq, int ldk, int ldv, int ldo, float scale, void* stream) {
+  return g3c::attn_fwd_sbhd(q, k, v, o, Lq, Lk, batch, heads, ldq, ldk, ldv, ldo, scale, (cudaStream_t)stream);
 }

@@ -267,6 +267,18 @@ __device__ __forceinline__ uint64_t make_sdesc_sw128(uint32_t smem_addr) {
   d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
+// Same for an MN-major tile (PTX ISA, "Matrix Descriptor Format"; the B operand of a wgmma with imm-trans-b = 1): each
+// 128-byte row holds 64 consecutive MN elements of one k, rows of consecutive k follow each other, so 8 k form one
+// 1024-B swizzle atom.  For the swizzled MN-major layouts LBO is the stride between the 64-element MN blocks of the atom
+// (`mn_block_bytes`) and SBO the stride between 8-k row groups (1024 B).
+__device__ __forceinline__ uint64_t make_sdesc_sw128_mn(uint32_t smem_addr, uint32_t mn_block_bytes) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
+  d |= static_cast<uint64_t>((mn_block_bytes >> 4) & 0x3FFFu) << 16;
+  d |= static_cast<uint64_t>(1024u >> 4) << 32;
+  d |= static_cast<uint64_t>(1) << 62;
+  return d;
+}
 // advance along K inside the 128-byte swizzle span: +bytes on the (unswizzled) start address
 __device__ __forceinline__ uint64_t sdesc_advance(uint64_t d, uint32_t bytes) {
   return d + static_cast<uint64_t>(bytes >> 4);

@@ -1,6 +1,7 @@
 """Thin torch-tensor wrappers over the per-operator C ABI entry points of Path D (used by the tests,
-and usable as drop-in operators, e.g. ``attention`` as an ``attn_op`` for the reference's
-``Attention(attn_op=...)`` seam, module/attention.py:136-139).  CUDA only; no fallback."""
+and usable as drop-in operators, e.g. ``attention_sbhd`` behind ``attention_op.DotProductAttention``, the
+``attn_op`` of the reference's ``Attention(attn_op=...)`` seam, module/attention.py:136-139).  CUDA only; no
+fallback."""
 from __future__ import annotations
 
 from typing import Optional
@@ -79,6 +80,48 @@ def attention(q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, heads: int, sc
     with torch.cuda.device(q.device):
         _lib.check(lib.g3c_attn_fwd(_lib.ptr(q), _lib.ptr(k), _lib.ptr(vt), _lib.ptr(o), Lq, Lk, heads, Dq, Dq, Dq,
                                     vt_chunk_len, scale, _lib.stream_ptr()), "g3c_attn_fwd")
+    return o
+
+
+def _token_stride(t: torch.Tensor, name: str) -> int:
+    """Leading dimension (elements) of an sbhd tensor viewed as [s, b*h*d]; ValueError unless the kernel can read it."""
+    if not t.is_cuda or t.dtype != torch.bfloat16:
+        raise ValueError(f"{name} must be a bf16 CUDA tensor, got {t.dtype} on {t.device}")
+    if t.dim() != 4 or t.shape[0] < 1 or t[0].numel() == 0:
+        raise ValueError(f"{name} must be a non-empty [s, b, h, d] tensor, got shape {tuple(t.shape)}")
+    if not t[0].is_contiguous():
+        raise ValueError(f"the (b, h, d) block of {name} must be contiguous, got strides {t.stride()}")
+    row = t[0].numel()
+    ld = t.stride(0) if t.shape[0] > 1 else row
+    if ld < row or ld % 8 != 0:
+        raise ValueError(f"the token stride of {name} ({ld}) must be a multiple of 8 and >= b*h*d = {row}")
+    if t.data_ptr() % 16 != 0:
+        raise ValueError(f"{name} must start on a 16-byte boundary")
+    return ld
+
+
+def attention_sbhd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Optional[float] = None) -> torch.Tensor:
+    """TE DotProductAttention(qkv_format="sbhd") semantics on the native kernel: q [sq, b, h, 128], k and v
+    [sk, b, h, 128] (V as given, any sq, sk >= 1) -> o [sq, b, h*128] = softmax(q k^T * scale) v per (batch, head).
+    scale defaults to 1/sqrt(128).  Unsupported shapes raise NotImplementedError, malformed tensors ValueError."""
+    if q.dim() == 4 and q.shape[-1] != 128:
+        raise NotImplementedError(f"head_dim {q.shape[-1]}: only 128 is implemented")
+    if q.dim() == 4 and k.dim() == 4 and k.shape[2] != q.shape[2]:
+        raise NotImplementedError(f"{k.shape[2]} key heads for {q.shape[2]} query heads: GQA is not implemented")
+    ldq, ldk, ldv = _token_stride(q, "q"), _token_stride(k, "k"), _token_stride(v, "v")
+    if k.shape != v.shape or k.shape[1:] != q.shape[1:]:
+        raise ValueError(f"q {tuple(q.shape)}, k {tuple(k.shape)} and v {tuple(v.shape)} must agree in (b, h, d) "
+                         "and k, v in s")
+    if not (q.device == k.device == v.device):
+        raise ValueError("q, k and v must be on one device")
+    sq, b, h, d = q.shape
+    o = torch.empty((sq, b, h * d), device=q.device, dtype=torch.bfloat16)
+    if scale is None:
+        scale = 128 ** -0.5
+    lib = _lib.load()
+    with torch.cuda.device(q.device):
+        _lib.check(lib.g3c_attn_fwd_sbhd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), sq, k.shape[0], b, h,
+                                         ldq, ldk, ldv, b * h * d, scale, _lib.stream_ptr()), "g3c_attn_fwd_sbhd")
     return o
 
 

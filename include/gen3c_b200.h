@@ -143,6 +143,16 @@ int g3c_gemm_norm_rope_bf16(const void* A, const void* B, void* D, int M, int N,
 int g3c_attn_fwd(const void* q, const void* k, const void* vt, void* o, int Lq, int Lk, int heads,
                  int ldq, int ldk, int ldo, int vt_chunk_len, float scale, void* stream);
 
+/* The same operator on the layout of TE DotProductAttention(qkv_format="sbhd") — the reference's `attn_op` seam
+ * (module/attention.py:136-139,288) — with V as given and any key count.
+ *   q [Lq][batch*heads*128] (ld ldq), k and v [Lk][batch*heads*128] (ld ldk, ldv), o [Lq][batch*heads*128] (ld ldo):
+ *   the token rows of [s, b, h, 128] tensors whose (b, h, d) block is contiguous, so batch x heads are one launch's
+ *   heads.  Lq, Lk >= 1 (no multiple-of-128 rule: the keys past Lk in the last KV tile are masked).  Leading
+ *   dimensions in elements, multiples of 8 and >= batch*heads*128; pointers 16-byte aligned; batch*heads <= 65535.
+ *   scale as in g3c_attn_fwd (1/sqrt(128) for TE's default; ln 2 when Q already carries softmax_scale * log2(e)). */
+int g3c_attn_fwd_sbhd(const void* q, const void* k, const void* v, void* o, int Lq, int Lk, int batch, int heads,
+                      int ldq, int ldk, int ldv, int ldo, float scale, void* stream);
+
 /* Profiling aid: when a device buffer of 3*64*8 uint64 is registered, the next g3c_attn_fwd launches run a
  * traced build of the kernel in which CTA (0,0) records clock64() stamps per KV step j (first 64 steps): roles 1/2 =
  * the two consumer warpgroups; slots 0 turn acquired, 1 MMAs of the step issued (S_j and P_{j-1} V_{j-1}), 2 S_j

@@ -1,7 +1,11 @@
 """Sustained timing of the attention kernel at the benchmark's self-attention shape (Lq = Lk = 56 320, 32 heads, head
 dim 128, scale = ln 2), long enough for a power-capped card to settle at its sustained clock.
 
-    python tools/attn_timing.py [--seconds 20] [--trace OUT.json]
+    python tools/attn_timing.py [--seconds 20] [--trace OUT.json] [--v-layout {vt,tokens}] [--lk LK]
+
+--v-layout vt (the default) times g3c_attn_fwd with V transposed, the engine's layout; tokens times g3c_attn_fwd_sbhd
+(gen3c_b200.ops.attention_sbhd, the TE-compatible operator) with V token-major like K.  --lk sets the key count
+(default 56 320; 512 is the cross-attention shape).
 
 The library is the one gen3c_b200 loads (GEN3C_B200_LIB selects another build), so two builds are compared by running
 this once per build, alternately.  Prints one JSON line: ms per launch, TFLOP/s, the share of the dense-bf16 peak at the
@@ -24,7 +28,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 L, HEADS = 56320, 32
-FLOP = 4.0 * L * L * 128 * HEADS  # Q K^T and P V, 2 FLOP per multiply-add
 
 
 def smi_sampler(samples, stop):
@@ -42,7 +45,13 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--seconds", type=float, default=20.0)
     ap.add_argument("--trace", default=None)
+    ap.add_argument("--v-layout", choices=["vt", "tokens"], default="vt")
+    ap.add_argument("--lk", type=int, default=L)
     args = ap.parse_args()
+    if args.trace and args.v_layout != "vt":
+        ap.error("--trace records the V^T kernel only")
+    Lk = args.lk
+    flop = 4.0 * L * Lk * 128 * HEADS  # Q K^T and P V, 2 FLOP per multiply-add
 
     import torch
 
@@ -51,12 +60,18 @@ def main():
     assert torch.cuda.is_available(), "attn_timing needs a CUDA device"
     dev = torch.device("cuda", 0)
     g = torch.Generator(device=dev).manual_seed(5)
-    q, k, v = ((torch.randn(L, HEADS * 128, device=dev, generator=g)).to(torch.bfloat16) for _ in range(3))
-    vt = v.T.contiguous()
+    q, k, v = ((torch.randn(n, HEADS * 128, device=dev, generator=g)).to(torch.bfloat16) for n in (L, Lk, Lk))
     scale = math.log(2.0)
+    if args.v_layout == "vt":
+        vt = v.T.contiguous()
 
-    def launch():
-        return ops.attention(q, k, vt, HEADS, scale=scale)
+        def launch():
+            return ops.attention(q, k, vt, HEADS, scale=scale)
+    else:
+        q4, k4, v4 = (t.view(-1, 1, HEADS, 128) for t in (q, k, v))
+
+        def launch():
+            return ops.attention_sbhd(q4, k4, v4, scale=scale)
 
     t_end = time.time() + 3.0  # warm-up: module load, then a few seconds toward the sustained clock
     while time.time() < t_end:
@@ -78,8 +93,9 @@ def main():
     stop.set()
     th.join()
     ms = statistics.median(times)
-    tflops = FLOP / (ms * 1e-3) / 1e12
-    out = {"lib": os.environ.get("GEN3C_B200_LIB", str(_lib.LIB_PATH)), "shape": f"{L}x{L}, {HEADS} heads, d=128",
+    tflops = flop / (ms * 1e-3) / 1e12
+    out = {"lib": os.environ.get("GEN3C_B200_LIB", str(_lib.LIB_PATH)), "shape": f"{L}x{Lk}, {HEADS} heads, d=128",
+           "v_layout": args.v_layout,
            "launches": 4 * len(times), "seconds": args.seconds, "ms_per_launch_median": ms,
            "ms_per_launch_min": min(times), "ms_per_launch_max": max(times), "tflops": tflops}
     if samples:
