@@ -72,6 +72,7 @@ SIGNATURES = {
     "g3c_device_info": (_I, [C.POINTER(_I), C.POINTER(_I), C.POINTER(_I)]),
     "g3c_render_create": (_I, [_I, _I, _I, C.POINTER(_P)]),
     "g3c_render_destroy": (_I, [_P]),
+    "g3c_render_set_deterministic": (_I, [_P, _I]),
     "g3c_forward_warp": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P]),
     "g3c_render_cache": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P]),
     "g3c_bilinear_splatting": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P]),

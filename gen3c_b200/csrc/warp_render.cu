@@ -102,8 +102,8 @@ struct ItemMap {
   int F;          // cameras (target frames) per batch element
   int src_bcast;  // 1: cache has a single frame broadcast over F targets
   int item0;      // first item of the current pass (foreground pass: blockIdx.y counts from here)
-  __device__ __forceinline__ int cam(int i) const { return (i + item0) / N; }
-  __device__ __forceinline__ int src(int i) const {
+  __host__ __device__ __forceinline__ int cam(int i) const { return (i + item0) / N; }
+  __host__ __device__ __forceinline__ int src(int i) const {
     const int j = i + item0;
     return src_bcast ? (j / (N * F)) * N + (j % N) : j;
   }
@@ -182,9 +182,9 @@ __global__ void __launch_bounds__(256) k_depth_max(const float* __restrict__ dep
 // ------------------------------------------------------------------------------------------------
 // pass 2: splat.  acc: [items_in_pass][H+2][W+2][4] = {c0*w, c1*w, c2*w, w};  accz: [..][H+2][W+2]
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void splat_pixel(float* __restrict__ acc, float* __restrict__ accz,
-                                            const SplatIdx& s, float z, float lz_max, float mask,
-                                            float v0, float v1, float v2, int W) {
+// The reference's splat weights of the nw, sw, ne, se corners (:623-646), IEEE divisions, expf and log1pf.
+__device__ __forceinline__ void corner_weights(const SplatIdx& s, float z, float lz_max, float mask, float& w_nw,
+                                               float& w_sw, float& w_ne, float& w_se) {
   // reference :623-634
   float dyf = __fsub_rn(1.0f, __fsub_rn(s.py, (float)s.fy));
   float dyc = __fsub_rn(1.0f, __fsub_rn((float)s.cy, s.py));
@@ -195,10 +195,17 @@ __device__ __forceinline__ void splat_pixel(float* __restrict__ acc, float* __re
   float e = __fmul_rn(__fdiv_rn(lz, __fadd_rn(lz_max, 1e-7f)), 50.0f);
   e = fminf(e, 80.0f);
   float dw = __fadd_rn(expf(e), 1e-7f);
-  float w_nw = __fdiv_rn(__fmul_rn(__fmul_rn(dyf, dxf), mask), dw);
-  float w_sw = __fdiv_rn(__fmul_rn(__fmul_rn(dyc, dxf), mask), dw);
-  float w_ne = __fdiv_rn(__fmul_rn(__fmul_rn(dyf, dxc), mask), dw);
-  float w_se = __fdiv_rn(__fmul_rn(__fmul_rn(dyc, dxc), mask), dw);
+  w_nw = __fdiv_rn(__fmul_rn(__fmul_rn(dyf, dxf), mask), dw);
+  w_sw = __fdiv_rn(__fmul_rn(__fmul_rn(dyc, dxf), mask), dw);
+  w_ne = __fdiv_rn(__fmul_rn(__fmul_rn(dyf, dxc), mask), dw);
+  w_se = __fdiv_rn(__fmul_rn(__fmul_rn(dyc, dxc), mask), dw);
+}
+
+__device__ __forceinline__ void splat_pixel(float* __restrict__ acc, float* __restrict__ accz,
+                                            const SplatIdx& s, float z, float lz_max, float mask,
+                                            float v0, float v1, float v2, int W) {
+  float w_nw, w_sw, w_ne, w_se;
+  corner_weights(s, z, lz_max, mask, w_nw, w_sw, w_ne, w_se);
   const int Wp = W + 2;
   size_t i_nw = (size_t)s.fy * Wp + s.fx, i_sw = (size_t)s.cy * Wp + s.fx;
   size_t i_ne = (size_t)s.fy * Wp + s.cx, i_se = (size_t)s.cy * Wp + s.cx;
@@ -394,6 +401,283 @@ __global__ void __launch_bounds__(256)
 }
 
 // ------------------------------------------------------------------------------------------------
+// pass 2, ordered (torch.use_deterministic_algorithms): the splat of ONE item without float atomics, bitwise
+// reproducible.  Every (source pixel, corner) pair is a record with id = corner * HW + source (corners nw, sw, ne, se
+// = 0..3) and key = its interior destination texel.  A stable LSD radix sort of (key, id) lists each texel's records
+// in ascending id, i.e. corner-major, then source row-major: the order of the reference's index_put_(accumulate=True)
+// under the deterministic flag (and of a sequential np.add.at).  One thread per texel then recomputes its records'
+// contributions and sums them sequentially in fp32 from 0.  Records with weight 0 or a destination in the cropped
+// 1-px ring change no output for finite inputs and are dropped by the key pass.  Integer shared-memory atomics only
+// count; every rank that decides an order comes from __match_any_sync / popc in warp, lane and block order.
+// ------------------------------------------------------------------------------------------------
+constexpr uint32_t RS_NONE = 0xFFFFFFFFu;  // dropped record
+constexpr int RS_BITS = 10, RS_DIGITS = 1 << RS_BITS;
+constexpr int RS_THREADS = 256, RS_WARPS = RS_THREADS / 32, RS_PER_THREAD = 16;
+constexpr int RS_TILE = RS_THREADS * RS_PER_THREAD;  // a warp ranks 32 * RS_PER_THREAD consecutive records
+constexpr int DET_BATCH = 8;                         // records whose contributions one thread computes at once
+
+// One item's splat inputs: projected points (forward_warp, render_cache) or a given flow (bilinear_splatting).
+struct DetItem {
+  const float* points;  // [HW][3], or NULL: flow / depth given
+  const float* w2c;     // [4][4] and [3][3] target camera (points only)
+  const float* K;
+  const float* flow;    // [2][HW] (flow only)
+  const float* depth;   // [HW] (flow only)
+  const float* image;   // [C][HW]
+  const float* mask;    // [HW] or NULL
+  const float* lz_max;  // the item's log-depth max
+  int C, H, W;
+};
+
+struct DetSrc {
+  float fx, fy, z, m, v0, v1, v2;
+};
+
+// the per-source arithmetic of k_splat_points (reference forward_warp :244-250) / k_splat_flow
+__device__ __forceinline__ DetSrc det_load(const DetItem& a, const Cam& c, int i) {
+  const int HW = a.H * a.W, y = i / a.W, x = i - y * a.W;
+  DetSrc s;
+  if (a.points) {
+    float qx, qy, qz;
+    project(c, a.points[3 * i], a.points[3 * i + 1], a.points[3 * i + 2], qx, qy, qz);
+    s.m = (a.mask ? a.mask[i] : 1.0f) * (qz > 0.0f ? 1.0f : 0.0f);
+    const float den = __fadd_rn(qz, 1e-7f);
+    s.fx = __fsub_rn(__fdiv_rn(qx, den), (float)x);
+    s.fy = __fsub_rn(__fdiv_rn(qy, den), (float)y);
+    s.z = qz;
+  } else {
+    s.fx = a.flow[i];
+    s.fy = a.flow[HW + i];
+    s.z = a.depth[i];
+    s.m = a.mask ? a.mask[i] : 1.0f;
+  }
+  s.v0 = a.image[i];
+  s.v1 = a.C > 1 ? a.image[HW + i] : 0.0f;
+  s.v2 = a.C > 2 ? a.image[2 * HW + i] : 0.0f;
+  return s;
+}
+
+__device__ __forceinline__ Cam det_cam(const DetItem& a) {
+  Cam c{};
+  if (a.points) c = load_cam(a.w2c, a.K);
+  return c;
+}
+
+// keys[corner * HW + i] = interior texel (y - 1) * W + (x - 1), or RS_NONE; optionally the flow of each source
+__global__ void __launch_bounds__(256) k_det_keys(DetItem a, uint32_t* __restrict__ keys, float* __restrict__ flow_out) {
+  const int H = a.H, W = a.W, HW = H * W;
+  const Cam c = det_cam(a);
+  const float lz_max = *a.lz_max;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += gridDim.x * blockDim.x) {
+    const int y = i / W, x = i - y * W;
+    const DetSrc s = det_load(a, c, i);
+    if (flow_out) {
+      flow_out[i] = s.fx;
+      flow_out[HW + i] = s.fy;
+    }
+    const SplatIdx si = splat_indices(s.fx, s.fy, x, y, W, H);
+    float w[4];
+    corner_weights(si, s.z, lz_max, s.m, w[0], w[1], w[2], w[3]);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int ty = (k & 1) ? si.cy : si.fy, tx = (k & 2) ? si.cx : si.fx;
+      const bool keep = w[k] != 0.0f && ty >= 1 && ty <= H && tx >= 1 && tx <= W;
+      keys[(size_t)k * HW + i] = keep ? (uint32_t)((ty - 1) * W + (tx - 1)) : RS_NONE;
+    }
+  }
+}
+
+__device__ __forceinline__ uint32_t rs_digit(uint32_t key, int shift) {
+  return key == RS_NONE ? RS_NONE : (key >> shift) & (RS_DIGITS - 1);
+}
+
+// n: the record count, from the host (first pass) or from the device (later passes, after dropping)
+__device__ __forceinline__ int rs_count(int n_host, const int* n_dev) { return n_dev ? *n_dev : n_host; }
+
+// hist[digit][block]: records of each digit in each block's tile
+__global__ void __launch_bounds__(RS_THREADS)
+    k_rs_hist(const uint32_t* __restrict__ keys, int n_host, const int* __restrict__ n_dev, int shift, int nblocks,
+              uint32_t* __restrict__ hist) {
+  __shared__ uint32_t h[RS_DIGITS];
+  for (int d = threadIdx.x; d < RS_DIGITS; d += RS_THREADS) h[d] = 0;
+  __syncthreads();
+  const int n = rs_count(n_host, n_dev);
+  const int lane = threadIdx.x & 31;
+  for (int j = threadIdx.x; j < RS_TILE; j += RS_THREADS) {
+    const int e = blockIdx.x * RS_TILE + j;
+    const uint32_t d = rs_digit(e < n ? keys[e] : RS_NONE, shift);
+    const uint32_t peers = __match_any_sync(0xffffffffu, d);
+    if (d != RS_NONE && lane == __ffs(peers) - 1) atomicAdd(&h[d], (uint32_t)__popc(peers));
+  }
+  __syncthreads();
+  for (int d = threadIdx.x; d < RS_DIGITS; d += RS_THREADS) hist[(size_t)d * nblocks + blockIdx.x] = h[d];
+}
+
+// exclusive scan over a block of RS_THREADS threads; *total = the sum of all v
+__device__ __forceinline__ uint32_t rs_block_scan(uint32_t v, uint32_t* total) {
+  __shared__ uint32_t ws[RS_WARPS];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  uint32_t x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) ws[w] = x;
+  __syncthreads();
+  uint32_t before = 0, all = 0;
+#pragma unroll
+  for (int k = 0; k < RS_WARPS; ++k) {
+    before += k < w ? ws[k] : 0u;
+    all += ws[k];
+  }
+  __syncthreads();
+  *total = all;
+  return before + x - v;
+}
+
+// one block per digit: hist[d][*] := exclusive scan over the blocks (block order); dtot[d] = the digit's total
+__global__ void __launch_bounds__(RS_THREADS)
+    k_rs_rowscan(uint32_t* __restrict__ hist, int nblocks, uint32_t* __restrict__ dtot) {
+  uint32_t* row = hist + (size_t)blockIdx.x * nblocks;
+  const int per = (nblocks + RS_THREADS - 1) / RS_THREADS;
+  const int b0 = min(threadIdx.x * per, nblocks), b1 = min(b0 + per, nblocks);
+  uint32_t s = 0;
+  for (int b = b0; b < b1; ++b) s += row[b];
+  uint32_t total;
+  uint32_t run = rs_block_scan(s, &total);
+  for (int b = b0; b < b1; ++b) {
+    const uint32_t t = row[b];
+    row[b] = run;
+    run += t;
+  }
+  if (threadIdx.x == 0) dtot[blockIdx.x] = total;
+}
+
+// Stable scatter of one radix pass.  Position = (records of smaller digits) + (records of this digit in earlier
+// blocks) + (in earlier warps of this block) + (in earlier 32-record chunks of this warp) + (in lower lanes).
+// ids_in == NULL: the first pass, id = position in keys_in.  Block 0 stores the number of records kept in *n_out.
+__global__ void __launch_bounds__(RS_THREADS)
+    k_rs_scatter(const uint32_t* __restrict__ keys_in, const uint32_t* __restrict__ ids_in, int n_host,
+                 const int* __restrict__ n_dev, int shift, int nblocks, const uint32_t* __restrict__ hist,
+                 const uint32_t* __restrict__ dtot, uint32_t* __restrict__ keys_out, uint32_t* __restrict__ ids_out,
+                 int* __restrict__ n_out) {
+  __shared__ uint32_t wcnt[RS_WARPS][RS_DIGITS];
+  __shared__ uint32_t dbase[RS_DIGITS];
+  constexpr int DPT = RS_DIGITS / RS_THREADS;
+  uint32_t t[DPT], s = 0;
+#pragma unroll
+  for (int k = 0; k < DPT; ++k) s += (t[k] = dtot[DPT * threadIdx.x + k]);
+  uint32_t total;
+  uint32_t run = rs_block_scan(s, &total);
+#pragma unroll
+  for (int k = 0; k < DPT; ++k) {
+    dbase[DPT * threadIdx.x + k] = run;
+    run += t[k];
+  }
+  if (n_out && blockIdx.x == 0 && threadIdx.x == 0) *n_out = (int)total;
+  for (int d = threadIdx.x; d < RS_WARPS * RS_DIGITS; d += RS_THREADS) (&wcnt[0][0])[d] = 0;
+  __syncthreads();
+  const int n = rs_count(n_host, n_dev);
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const uint32_t lower = (1u << lane) - 1u;
+  const int base = blockIdx.x * RS_TILE + w * 32 * RS_PER_THREAD + lane;
+  uint32_t key[RS_PER_THREAD], rank[RS_PER_THREAD];
+#pragma unroll
+  for (int c = 0; c < RS_PER_THREAD; ++c) {
+    const int e = base + 32 * c;
+    key[c] = e < n ? keys_in[e] : RS_NONE;
+    const uint32_t d = rs_digit(key[c], shift);
+    const uint32_t peers = __match_any_sync(0xffffffffu, d);
+    rank[c] = d != RS_NONE ? wcnt[w][d] + __popc(peers & lower) : 0u;
+    __syncwarp();
+    if (d != RS_NONE && lane == __ffs(peers) - 1) wcnt[w][d] += __popc(peers);
+    __syncwarp();
+  }
+  __syncthreads();
+  for (int d = threadIdx.x; d < RS_DIGITS; d += RS_THREADS) {
+    uint32_t r = dbase[d] + hist[(size_t)d * nblocks + blockIdx.x];
+#pragma unroll
+    for (int k = 0; k < RS_WARPS; ++k) {
+      const uint32_t c = wcnt[k][d];
+      wcnt[k][d] = r;
+      r += c;
+    }
+  }
+  __syncthreads();
+#pragma unroll
+  for (int c = 0; c < RS_PER_THREAD; ++c) {
+    const uint32_t d = rs_digit(key[c], shift);
+    if (d == RS_NONE) continue;
+    const int e = base + 32 * c;
+    const uint32_t pos = wcnt[w][d] + rank[c];
+    keys_out[pos] = key[c];
+    ids_out[pos] = ids_in ? ids_in[e] : (uint32_t)e;
+  }
+}
+
+// seg[texel] = [first, last + 1) of its records in the sorted keys (seg zeroed beforehand: empty texels stay [0, 0))
+__global__ void __launch_bounds__(256)
+    k_det_bounds(const uint32_t* __restrict__ keys, const int* __restrict__ n_dev, uint2* __restrict__ seg) {
+  const int n = *n_dev;
+  for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) {
+    const uint32_t k = keys[p];
+    if (p == 0 || keys[p - 1] != k) seg[k].x = p;
+    if (p == n - 1 || keys[p + 1] != k) seg[k].y = p + 1;
+  }
+}
+
+// One thread per interior texel: its records' contributions summed in sorted order, written to the padded acc / accz
+// layout k_normalise reads (every interior texel is written, so the planes need no clearing).
+__global__ void __launch_bounds__(256)
+    k_det_accum(DetItem a, const uint32_t* __restrict__ ids, const uint2* __restrict__ seg, float* __restrict__ acc,
+                float* __restrict__ accz) {
+  const int H = a.H, W = a.W, HW = H * W;
+  const Cam c = det_cam(a);
+  const float lz_max = *a.lz_max;
+  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < HW; t += gridDim.x * blockDim.x) {
+    const uint2 sg = seg[t];
+    float s0 = 0.0f, s1 = 0.0f, s2 = 0.0f, sw = 0.0f, sz = 0.0f;
+    for (uint32_t p0 = sg.x; p0 < sg.y; p0 += DET_BATCH) {
+      // the contributions of a batch are independent: compute them together, add them in order
+      float c0[DET_BATCH], c1[DET_BATCH], c2[DET_BATCH], cw[DET_BATCH], cz[DET_BATCH];
+#pragma unroll
+      for (int j = 0; j < DET_BATCH; ++j) {
+        c0[j] = c1[j] = c2[j] = cw[j] = cz[j] = 0.0f;
+        if (p0 + j < sg.y) {
+          const uint32_t id = ids[p0 + j];
+          const int corner = (int)(id / (uint32_t)HW), i = (int)(id - (uint32_t)corner * HW);
+          const int y = i / W, x = i - y * W;
+          const DetSrc s = det_load(a, c, i);
+          const SplatIdx si = splat_indices(s.fx, s.fy, x, y, W, H);
+          float w[4];
+          corner_weights(si, s.z, lz_max, s.m, w[0], w[1], w[2], w[3]);
+          const float wt = corner == 0 ? w[0] : corner == 1 ? w[1] : corner == 2 ? w[2] : w[3];
+          c0[j] = __fmul_rn(s.v0, wt);
+          c1[j] = __fmul_rn(s.v1, wt);
+          c2[j] = __fmul_rn(s.v2, wt);
+          cw[j] = wt;
+          cz[j] = __fmul_rn(s.z, wt);
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < DET_BATCH; ++j)
+        if (p0 + j < sg.y) {
+          s0 = __fadd_rn(s0, c0[j]);
+          s1 = __fadd_rn(s1, c1[j]);
+          s2 = __fadd_rn(s2, c2[j]);
+          sw = __fadd_rn(sw, cw[j]);
+          sz = __fadd_rn(sz, cz[j]);
+        }
+    }
+    const int ty = t / W, tx = t - ty * W;
+    const size_t j = (size_t)(ty + 1) * (W + 2) + (tx + 1);
+    reinterpret_cast<float4*>(acc)[j] = make_float4(s0, s1, s2, sw);
+    if (accz) accz[j] = sz;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // pass 3: crop + normalise (reference :680-695)
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
@@ -547,6 +831,16 @@ struct g3c_render {
   float* accz;  // [max_items][H+2][W+2]
   float* gmax;  // per-group maxima
   int gmax_cap;
+  // ordered splat (g3c_render_set_deterministic); the workspace is allocated when it is first enabled
+  int det;
+  uint32_t* rs;         // the one allocation below
+  uint32_t* keys[2];    // [4 H W] each: radix sort ping-pong
+  uint32_t* ids[2];
+  uint32_t* hist;       // [RS_DIGITS][rs_blocks]
+  uint32_t* dtot;       // [RS_DIGITS]
+  uint2* seg;           // [H W] record range of each texel
+  int* count;           // records kept
+  int rs_blocks;
 };
 
 
@@ -866,7 +1160,57 @@ int g3c_render_destroy(g3c_render_t* r) {
   cudaFree(r->acc);
   cudaFree(r->accz);
   cudaFree(r->gmax);
+  cudaFree(r->rs);
   delete r;
+  return G3C_OK;
+}
+
+int g3c_render_set_deterministic(g3c_render_t* r, int on) {
+  G3C_REQUIRE(r, "render_set_deterministic: null handle");
+  if (on && !r->rs) {
+    const size_t HW = (size_t)r->H * r->W, n4 = 4 * HW;
+    G3C_REQUIRE(n4 <= (size_t)INT32_MAX, "render_set_deterministic: %d x %d frames are too large", r->H, r->W);
+    const int blocks = (int)((n4 + RS_TILE - 1) / RS_TILE);
+    // keys x2 | ids x2 | hist | dtot | seg | count (every part starts at an even word: seg is 8-byte aligned)
+    const size_t words = 4 * n4 + (size_t)RS_DIGITS * blocks + RS_DIGITS + 2 * HW + 2;
+    uint32_t* buf = nullptr;
+    G3C_CUDA(cudaMalloc(&buf, words * sizeof(uint32_t)));
+    r->rs = buf;
+    r->rs_blocks = blocks;
+    r->keys[0] = buf;
+    r->keys[1] = buf + n4;
+    r->ids[0] = buf + 2 * n4;
+    r->ids[1] = buf + 3 * n4;
+    r->hist = buf + 4 * n4;
+    r->dtot = r->hist + (size_t)RS_DIGITS * blocks;
+    r->seg = reinterpret_cast<uint2*>(r->dtot + RS_DIGITS);
+    r->count = reinterpret_cast<int*>(r->seg + HW);
+  }
+  r->det = on ? 1 : 0;
+  return G3C_OK;
+}
+
+// The ordered splat of one item (k_det_keys .. k_det_accum) into one acc / accz plane.
+static int det_splat_item(g3c_render* r, const DetItem& a, float* acc, float* accz, float* flow_out, cudaStream_t st) {
+  const int HW = r->H * r->W, n4 = 4 * HW;
+  int bits = 1;
+  while ((1LL << bits) < HW) ++bits;
+  const int passes = (bits + RS_BITS - 1) / RS_BITS;
+  // pass p reads buffer (p + 1) & 1 and writes p & 1; the keys pass writes buffer 1, the ids of pass 0 are implicit
+  k_det_keys<<<px_grid(HW, 1), 256, 0, st>>>(a, r->keys[1], flow_out);
+  for (int p = 0; p < passes; ++p) {
+    const int in = (p + 1) & 1, out = p & 1;
+    const int* n_dev = p ? r->count : nullptr;
+    k_rs_hist<<<r->rs_blocks, RS_THREADS, 0, st>>>(r->keys[in], n4, n_dev, RS_BITS * p, r->rs_blocks, r->hist);
+    k_rs_rowscan<<<RS_DIGITS, RS_THREADS, 0, st>>>(r->hist, r->rs_blocks, r->dtot);
+    k_rs_scatter<<<r->rs_blocks, RS_THREADS, 0, st>>>(r->keys[in], p ? r->ids[in] : nullptr, n4, n_dev, RS_BITS * p,
+                                                      r->rs_blocks, r->hist, r->dtot, r->keys[out], r->ids[out],
+                                                      p ? nullptr : r->count);
+  }
+  const int last = (passes - 1) & 1;
+  G3C_CUDA(cudaMemsetAsync(r->seg, 0, sizeof(uint2) * HW, st));
+  k_det_bounds<<<px_grid(n4, 1), 256, 0, st>>>(r->keys[last], r->count, r->seg);
+  k_det_accum<<<px_grid(HW, 1), 256, 0, st>>>(a, r->ids[last], r->seg, acc, accz);
   return G3C_OK;
 }
 
@@ -895,23 +1239,35 @@ static int render_items(g3c_render* r, const float* points, const float* image, 
   size_t plane = (size_t)(H + 2) * (W + 2);
   for (int i0 = 0; i0 < n_items; i0 += r->max_items) {
     int n = n_items - i0 < r->max_items ? n_items - i0 : r->max_items;
-    G3C_CUDA(cudaMemsetAsync(r->acc, 0, plane * 4 * sizeof(float) * n, st));
-    if (want_depth) G3C_CUDA(cudaMemsetAsync(r->accz, 0, plane * sizeof(float) * n, st));
-    // G3C_SPLAT=ref: the round-1 one-pixel-per-thread kernel with the reference's exact weight arithmetic (A/B runs)
-    static int fast = -1;
-    if (fast < 0) {
-      const char* e = getenv("G3C_SPLAT");
-      fast = !(e && e[0] == 'r');
+    if (r->det) {
+      for (int j = 0; j < n; ++j) {
+        const int item = i0 + j, src = map.src(item), cam = map.cam(item);
+        const DetItem a{points + (size_t)src * HW * 3, w2c + 16 * cam, K + 9 * cam, nullptr, nullptr,
+                        image + (size_t)src * C * HW, mask ? mask + (size_t)src * HW : nullptr, r->gmax + item / group,
+                        C, H, W};
+        const int rc = det_splat_item(r, a, r->acc + plane * 4 * j, want_depth ? r->accz + plane * j : nullptr,
+                                      flow_out ? flow_out + (size_t)item * 2 * HW : nullptr, st);
+        if (rc != G3C_OK) return rc;
+      }
+    } else {
+      G3C_CUDA(cudaMemsetAsync(r->acc, 0, plane * 4 * sizeof(float) * n, st));
+      if (want_depth) G3C_CUDA(cudaMemsetAsync(r->accz, 0, plane * sizeof(float) * n, st));
+      // G3C_SPLAT=ref: the round-1 one-pixel-per-thread kernel with the reference's exact weight arithmetic (A/B runs)
+      static int fast = -1;
+      if (fast < 0) {
+        const char* e = getenv("G3C_SPLAT");
+        fast = !(e && e[0] == 'r');
+      }
+      const bool aligned = (W % 4 == 0) && ((reinterpret_cast<uintptr_t>(points) | reinterpret_cast<uintptr_t>(image) |
+                                             reinterpret_cast<uintptr_t>(mask) | reinterpret_cast<uintptr_t>(flow_out)) % 16 == 0);
+      if (fast && aligned)
+        k_splat_points4<<<px_grid(HW / 4, n), 256, 0, st>>>(points, image, mask, w2c, K, map, i0, C, H, W, group, r->gmax,
+                                                            r->acc, want_depth ? r->accz : nullptr, flow_out);
+      else
+        k_splat_points<<<px_grid(HW, n), 256, 0, st>>>(points, image, mask, w2c, K, map, i0, C, H, W,
+                                                       group, r->gmax, r->acc,
+                                                       want_depth ? r->accz : nullptr, flow_out);
     }
-    const bool aligned = (W % 4 == 0) && ((reinterpret_cast<uintptr_t>(points) | reinterpret_cast<uintptr_t>(image) |
-                                           reinterpret_cast<uintptr_t>(mask) | reinterpret_cast<uintptr_t>(flow_out)) % 16 == 0);
-    if (fast && aligned)
-      k_splat_points4<<<px_grid(HW / 4, n), 256, 0, st>>>(points, image, mask, w2c, K, map, i0, C, H, W, group, r->gmax,
-                                                          r->acc, want_depth ? r->accz : nullptr, flow_out);
-    else
-      k_splat_points<<<px_grid(HW, n), 256, 0, st>>>(points, image, mask, w2c, K, map, i0, C, H, W,
-                                                     group, r->gmax, r->acc,
-                                                     want_depth ? r->accz : nullptr, flow_out);
     k_normalise<<<px_grid(HW, n), 256, 0, st>>>(r->acc, want_depth ? r->accz : nullptr, i0, C, H,
                                                 W, is_image, out, mask_out,
                                                 want_depth ? depth_out : nullptr);
@@ -962,9 +1318,19 @@ int g3c_bilinear_splatting(g3c_render_t* r, const float* frame, const float* mas
   size_t plane = (size_t)(H + 2) * (W + 2);
   for (int i0 = 0; i0 < b; i0 += r->max_items) {
     int n = b - i0 < r->max_items ? b - i0 : r->max_items;
-    G3C_CUDA(cudaMemsetAsync(r->acc, 0, plane * 4 * sizeof(float) * n, st));
-    k_splat_flow<<<px_grid(HW, n), 256, 0, st>>>(frame, mask, depth, flow, i0, C, H, W, r->gmax,
-                                                 r->acc);
+    if (r->det) {
+      for (int j = 0; j < n; ++j) {
+        const size_t item = i0 + j;
+        const DetItem a{nullptr, nullptr, nullptr, flow + item * 2 * HW, depth + item * HW, frame + item * C * HW,
+                        mask ? mask + item * HW : nullptr, r->gmax, C, H, W};
+        const int rc = det_splat_item(r, a, r->acc + plane * 4 * j, nullptr, nullptr, st);
+        if (rc != G3C_OK) return rc;
+      }
+    } else {
+      G3C_CUDA(cudaMemsetAsync(r->acc, 0, plane * 4 * sizeof(float) * n, st));
+      k_splat_flow<<<px_grid(HW, n), 256, 0, st>>>(frame, mask, depth, flow, i0, C, H, W, r->gmax,
+                                                   r->acc);
+    }
     k_normalise<<<px_grid(HW, n), 256, 0, st>>>(r->acc, nullptr, i0, C, H, W, is_image, out,
                                                 mask_out, nullptr);
   }

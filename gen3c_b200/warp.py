@@ -16,18 +16,23 @@ _workspaces: dict = {}
 
 
 def _workspace(h: int, w: int, device: torch.device, max_items: int = 4):
-    """One render workspace per (H, W, device): accumulation buffers for `max_items` frames."""
+    """One render workspace per (H, W, device): accumulation buffers for `max_items` frames.
+    Under torch.use_deterministic_algorithms(True) it splats in the reference's fixed order (bitwise reproducible,
+    as torch's index_put_(accumulate=True) is under that flag); otherwise with the faster float atomics."""
     key = (h, w, device.index, max_items)
+    lib = _lib.load()
     ws = _workspaces.get(key)
     if ws is None:
         import ctypes as C
 
-        lib = _lib.load()
         handle = C.c_void_p()
         with torch.cuda.device(device):
             _lib.check(lib.g3c_render_create(h, w, max_items, C.byref(handle)), "g3c_render_create")
         ws = handle
         _workspaces[key] = ws
+    with torch.cuda.device(device):
+        _lib.check(lib.g3c_render_set_deterministic(ws, 1 if torch.are_deterministic_algorithms_enabled() else 0),
+                   "g3c_render_set_deterministic")
     return ws
 
 

@@ -6,7 +6,7 @@
  * reproduces.  Conventions: every pointer is a DEVICE pointer owned by the caller unless noted;
  * `stream` is a cudaStream_t passed as void*; functions enqueue on that stream and return
  * immediately; return 0 on success, <0 on error (G3C_E*), message via g3c_last_error() (thread
- * local).  No hidden allocations after a *_create / *_set_shape call.  Handles are not thread
+ * local).  No hidden allocations after a *_create / *_set_shape / *_set_deterministic call.  Handles are not thread
  * safe; distinct handles are independent.  There is no CPU fallback anywhere in this library.
  */
 #ifndef GEN3C_B200_H_
@@ -37,6 +37,16 @@ typedef struct g3c_render g3c_render_t;
  * resident between the splat and the normalise pass. */
 int g3c_render_create(int H, int W, int max_items_per_pass, g3c_render_t** out);
 int g3c_render_destroy(g3c_render_t* r);
+
+/* on != 0: g3c_forward_warp, g3c_render_cache and g3c_bilinear_splatting on this handle splat in a fixed order and are
+ * bitwise reproducible whatever the pass size or the run (torch.use_deterministic_algorithms(True) for the
+ * reference's index_put_(accumulate=True)).  Each destination texel sums its contributions sequentially in fp32 from
+ * 0, corner-major (nw, sw, ne, se, reference :659-675), then in ascending source pixel, with the reference's weight
+ * arithmetic; no float atomics.  The first enable allocates the sort workspace, about 76 B per pixel of one frame
+ * (69 MB at 704 x 1280); g3c_render_destroy frees it.  on = 0 returns to the default atomic splat.
+ * Every other Path R entry point is deterministic already: the log-depth maxima and the foreground z-buffer are
+ * atomicMax / atomicMin on float bits, which do not depend on order, and every other output has one writer. */
+int g3c_render_set_deterministic(g3c_render_t* r, int on);
 
 #define G3C_WARP_RENDER_DEPTH 1 /* also splat z (forward_warp render_depth=True)            */
 #define G3C_WARP_NOT_IMAGE 2    /* is_image=False: fill 0 instead of -1, no clamp to [-1,1] */
