@@ -81,7 +81,7 @@ __global__ void __launch_bounds__(256)
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
     k_rmsnorm_rope(__nv_bfloat16* __restrict__ qk, int ld, int L, int heads,
-                   const float* __restrict__ gamma, const float* __restrict__ cs, float eps, PeerDst peers) {
+                   const float* __restrict__ gamma, const float* __restrict__ cs, float eps) {
   const int lane = threadIdx.x & 31;
   const long long wid = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (wid >= (long long)L * heads) return;
@@ -107,20 +107,8 @@ __global__ void __launch_bounds__(256)
     float m0 = b0 * co.x + a0 * si.x, m1 = b1 * co.y + a1 * si.y;
     a0 = n0; a1 = n1; b0 = m0; b1 = m1;
   }
-  const __nv_bfloat162 o0 = __floats2bfloat162_rn(a0, a1), o1 = __floats2bfloat162_rn(b0, b1);
-  *reinterpret_cast<__nv_bfloat162*>(p + 2 * lane) = o0;
-  *reinterpret_cast<__nv_bfloat162*>(p + 64 + 2 * lane) = o1;
-  // fused all-gather of the normalised keys: same offsets in the peers' buffers (NVLink posted writes)
-  const size_t off = (size_t)tok * ld + head * 128;
-  // (static indices only: a dynamically indexed kernel parameter would be copied to local memory by every thread)
-#pragma unroll
-  for (int i = 0; i < 7; ++i) {
-    if (i < peers.n) {
-      __nv_bfloat16* r = reinterpret_cast<__nv_bfloat16*>(peers.ptr[i]) + off;
-      *reinterpret_cast<__nv_bfloat162*>(r + 2 * lane) = o0;
-      *reinterpret_cast<__nv_bfloat162*>(r + 64 + 2 * lane) = o1;
-    }
-  }
+  *reinterpret_cast<__nv_bfloat162*>(p + 2 * lane) = __floats2bfloat162_rn(a0, a1);
+  *reinterpret_cast<__nv_bfloat162*>(p + 64 + 2 * lane) = __floats2bfloat162_rn(b0, b1);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -352,12 +340,10 @@ int ln_modulate(float* x, const __nv_bfloat16* pos, const float* shift, const fl
 }
 
 int rmsnorm_rope(__nv_bfloat16* qk, int ld, int L, int heads, const float* gamma, const float* cs,
-                 float eps, cudaStream_t st, const PeerDst* peers) {
-  PeerDst pd;
-  if (peers) pd = *peers;
+                 float eps, cudaStream_t st) {
   long long warps = (long long)L * heads;
   int blocks = (int)((warps + 7) / 8);
-  k_rmsnorm_rope<<<blocks, 256, 0, st>>>(qk, ld, L, heads, gamma, cs, eps, pd);
+  k_rmsnorm_rope<<<blocks, 256, 0, st>>>(qk, ld, L, heads, gamma, cs, eps);
   G3C_CUDA(cudaGetLastError());
   return G3C_OK;
 }

@@ -114,7 +114,6 @@ struct g3c_dit {
   // default CP mode: fused projection -> all-gather through NVLink peer memory.  One cudaMalloc'd region per
   // rank, IPC-mapped by every peer: K / V^T of all ranks, double buffered by layer parity, plus arrival flags.
   bool cp_p2p = true;
-  bool cp_push_sm = false;  // G3C_CP_PUSH=sm: peer stores from the producing kernels; default: copy engines
   void* cp_region = nullptr;
   size_t cp_region_bytes = 0, off_k[2] = {0, 0}, off_vt[2] = {0, 0}, off_flags = 0;
   void* peer_base[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
@@ -275,14 +274,11 @@ static int resolve(g3c_dit* h, cudaStream_t st) {
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
-// Publish "my K / V^T slices of layer `seq` have landed" in every rank's flag array.  Launched after the producer
-// kernels on the same stream (their peer writes are complete at kernel completion); release at system scope.
-__global__ void k_cp_signal(PeerDst slots, uint32_t seq) {
-  const int r = threadIdx.x;
-  if (r < slots.n) {
-    __threadfence_system();
-    asm volatile("st.release.sys.global.u32 [%0], %1;\n" ::"l"(slots.ptr[r]), "r"(seq) : "memory");
-  }
+// Publish "my output of step `seq` has landed" in the CFG partner's flag.  Launched after the copy into the partner's
+// memory on the same stream (complete when this kernel starts); release at system scope.
+__global__ void k_cp_signal(uint32_t* flag, uint32_t seq) {
+  __threadfence_system();
+  asm volatile("st.release.sys.global.u32 [%0], %1;\n" ::"l"(flag), "r"(seq) : "memory");
 }
 
 // Stream-ordered wait for a peer's flag (CFG-parallel output exchange): one warp polls with system-scope acquire loads.
@@ -353,35 +349,15 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
   const int D = c.model_channels, R = c.adaln_lora_dim, F = c.ffn_dim, L = h->L, heads = c.num_heads;
   const int Lk_all = L * h->cp_size;
   const float attn_scale = 0.6931471805599453f;  // ln 2: 1/sqrt(128) * log2(e) is folded into the query RMSNorm gain
-  // to_q / to_k: Linear + per-head RMSNorm (+ RoPE).  Fused into the GEMM epilogue (G3C_FUSE_NORM_ROPE, default on):
-  // the norm and the rotation act on the fp32 accumulators in registers and the [tokens, D] bf16 round trip of a separate
-  // pass disappears.
-  static int fuse_nr = -1;
-  if (fuse_nr < 0) {
-    const char* e = getenv("G3C_FUSE_NORM_ROPE");
-    fuse_nr = e ? atoi(e) != 0 : 1;
-  }
-  auto proj_norm_rope = [&](const void* a, const void* w, __nv_bfloat16* out, int M, int Kin,
-                            const float* gamma, const float* cs, int& launches) -> int {
-    if (fuse_nr) {
-      NormRope nr;
-      nr.gamma = gamma;
-      nr.cs = cs;
-      nr.eps = 1e-6f;
-      TRY(prof_mark(h, CAT_GEMM, true, st));
-      TRY(gemm_bf16(a, w, out, M, D, Kin, Kin, Kin, D, G3C_EPI_BF16, nullptr, 0, st, nullptr, &nr));
-      TRY(prof_mark(h, CAT_GEMM, false, st));
-      launches += 1;
-    } else {
-      TRY(prof_mark(h, CAT_GEMM, true, st));
-      TRY(gemm_bf16(a, w, out, M, D, Kin, Kin, Kin, D, G3C_EPI_BF16, nullptr, 0, st));
-      TRY(prof_mark(h, CAT_GEMM, false, st));
-      TRY(prof_mark(h, CAT_ELTWISE, true, st));
-      TRY(rmsnorm_rope(out, D, M, heads, gamma, cs, 1e-6f, st));
-      TRY(prof_mark(h, CAT_ELTWISE, false, st));
-      launches += 2;
-    }
-    return G3C_OK;
+  // to_q / to_k: Linear + per-head RMSNorm (+ RoPE), fused into the GEMM epilogue: the norm and the rotation act on the
+  // fp32 accumulators in registers, so the projection never round-trips [tokens, D] bf16 through a separate pass.
+  auto proj_norm_rope = [&](const void* a, const void* w, __nv_bfloat16* out, int M, int Kin, const float* gamma,
+                            const float* cs) {
+    NormRope nr;
+    nr.gamma = gamma;
+    nr.cs = cs;
+    nr.eps = 1e-6f;
+    return gemm_bf16(a, w, out, M, D, Kin, Kin, Kin, D, G3C_EPI_BF16, nullptr, 0, st, &nr);
   };
   int n = 0;
 
@@ -424,9 +400,12 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
       const float* m = h->mods + (size_t)(i * 3 + 0) * 3 * D;
       K(CAT_ELTWISE, ln_modulate(h->x, h->pos, m, m + D, h->xn, L, D, 1e-6f, st));   // + abs-pos add
       if (h->cp_size > 1 && h->cp_p2p) {
-        // fused projection -> all-gather: every rank stores its K / V^T slice straight into every peer's buffer
-        // (GEMM epilogue / RMSNorm-RoPE pass, NVLink posted writes), then raises a flag; attention starts on the
-        // local chunk at once and picks up the remote chunks as their flags arrive.
+        // all-gather through peer memory: every rank produces its K / V^T slice locally, then the copy engines push
+        // it into every peer's buffer on a side stream and raise a flag there, while this stream already runs the Q
+        // projection and attention over the local chunk; attention picks up the remote chunks as their flags arrive.
+        // Peer (me-1) is served first, then (me-2), ...: rank c consumes chunk c+1 first, so its k-th remote chunk is
+        // the k-th push of its producer.  The flag that opens the chunk on a peer follows that peer's two copies on the
+        // same stream (a 4-byte copy from a pinned ring: no kernel, see seq_ring).
         G3C_REQUIRE(h->peers_open, "dit_forward: context-parallel peers not imported (g3c_dit_cp_import)");
         const uint32_t seq = ++h->kv_seq;
         const int set = seq & 1, me = h->cp_rank;
@@ -436,46 +415,23 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
         __nv_bfloat16* vb = (__nv_bfloat16*)(reg + h->off_vt[set]);
         __nv_bfloat16* kl = kb + (size_t)me * L * D;
         __nv_bfloat16* vl = vb + (size_t)me * L * D;
-        PeerDst pk, pv, pf;
-        for (int r = 0; r < h->cp_size; ++r) {
+        K(CAT_GEMM, proj_norm_rope(h->xn, s.wk, kl, L, D, s.gk, h->rope));
+        K(CAT_GEMM, gemm_bf16(s.wv, h->xn, vl, D, L, D, D, D, L, G3C_EPI_BF16, nullptr, 0, st));  // V^T
+        G3C_CUDA(cudaEventRecord(h->ev_kv, st));
+        G3C_CUDA(cudaStreamWaitEvent(h->comm_stream, h->ev_kv, 0));
+        uint32_t* slot = h->seq_ring + (seq % g3c_dit::kSeqRing);
+        *slot = seq;  // read by the copy engine when the copies queued before it have completed
+        for (int i2 = 1; i2 < h->cp_size; ++i2) {
+          const int r = (me - i2 + h->cp_size) % h->cp_size;
           char* pb = (char*)h->peer_base[r];
-          pf.ptr[pf.n++] = pb + h->off_flags + (size_t)(set * 8 + me) * 4;
-          if (r == me) continue;
-          pk.ptr[pk.n++] = pb + h->off_k[set] + (size_t)me * slice;
-          pv.ptr[pv.n++] = pb + h->off_vt[set] + (size_t)me * slice;
+          G3C_CUDA(cudaMemcpyAsync(pb + h->off_k[set] + (size_t)me * slice, kl, slice, cudaMemcpyDeviceToDevice,
+                                   h->comm_stream));
+          G3C_CUDA(cudaMemcpyAsync(pb + h->off_vt[set] + (size_t)me * slice, vl, slice, cudaMemcpyDeviceToDevice,
+                                   h->comm_stream));
+          G3C_CUDA(cudaMemcpyAsync(pb + h->off_flags + (size_t)(set * 8 + me) * 4, slot, 4, cudaMemcpyHostToDevice,
+                                   h->comm_stream));
         }
-        if (h->cp_push_sm) {
-          // variant A (G3C_CP_PUSH=sm): the producing kernels themselves store every tile to all peers
-          K(CAT_GEMM, gemm_bf16(h->xn, s.wk, kl, L, D, D, D, D, D, G3C_EPI_BF16, nullptr, 0, st));
-          K(CAT_COMM, rmsnorm_rope(kl, D, L, heads, s.gk, h->rope, 1e-6f, st, &pk));
-          K(CAT_COMM, gemm_bf16(s.wv, h->xn, vl, D, L, D, D, D, L, G3C_EPI_BF16, nullptr, 0, st, &pv));  // V^T
-          k_cp_signal<<<1, 32, 0, st>>>(pf, seq);
-          G3C_CUDA(cudaGetLastError());
-          ++n;
-        } else {
-          // default: produce locally, then the copy engines push the two slices to every peer on a side stream while
-          // this stream already runs the Q projection and attention over the local chunk.  Peer (me-1) is served
-          // first, then (me-2), ...: rank c consumes chunk c+1 first, so its k-th remote chunk is the k-th push of
-          // its producer.  The flag that opens the chunk on a peer follows that peer's two copies on the same stream
-          // (a 4-byte copy from a pinned ring: no kernel, see seq_ring).
-          TRY(proj_norm_rope(h->xn, s.wk, kl, L, D, s.gk, h->rope, n));
-          K(CAT_GEMM, gemm_bf16(s.wv, h->xn, vl, D, L, D, D, D, L, G3C_EPI_BF16, nullptr, 0, st));  // V^T
-          G3C_CUDA(cudaEventRecord(h->ev_kv, st));
-          G3C_CUDA(cudaStreamWaitEvent(h->comm_stream, h->ev_kv, 0));
-          uint32_t* slot = h->seq_ring + (seq % g3c_dit::kSeqRing);
-          *slot = seq;  // read by the copy engine when the copies queued before it have completed
-          for (int i2 = 1; i2 < h->cp_size; ++i2) {
-            const int r = (me - i2 + h->cp_size) % h->cp_size;
-            char* pb = (char*)h->peer_base[r];
-            G3C_CUDA(cudaMemcpyAsync(pb + h->off_k[set] + (size_t)me * slice, kl, slice, cudaMemcpyDeviceToDevice,
-                                     h->comm_stream));
-            G3C_CUDA(cudaMemcpyAsync(pb + h->off_vt[set] + (size_t)me * slice, vl, slice, cudaMemcpyDeviceToDevice,
-                                     h->comm_stream));
-            G3C_CUDA(cudaMemcpyAsync(pb + h->off_flags + (size_t)(set * 8 + me) * 4, slot, 4, cudaMemcpyHostToDevice,
-                                     h->comm_stream));
-          }
-        }
-        TRY(proj_norm_rope(h->xn, s.wq, h->q, L, D, s.gq, h->rope, n));
+        K(CAT_GEMM, proj_norm_rope(h->xn, s.wq, h->q, L, D, s.gq, h->rope));
         ChunkGate gate;
         gate.flags = (const uint32_t*)(reg + h->off_flags) + set * 8;
         gate.seq = seq;
@@ -484,7 +440,7 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
         h->wait_cta_launches = (double)((L + ATT_ROWS_PER_CTA - 1) / ATT_ROWS_PER_CTA) * heads;  // CTAs of one gated launch
         K(CAT_ATTN_SELF, attn_fwd(h->q, kb, vb, h->att, L, Lk_all, heads, D, D, D, L, attn_scale, st, &gate));
       } else {
-        TRY(proj_norm_rope(h->xn, s.wk, k_loc, L, D, s.gk, h->rope, n));
+        K(CAT_GEMM, proj_norm_rope(h->xn, s.wk, k_loc, L, D, s.gk, h->rope));
         K(CAT_GEMM, gemm_bf16(s.wv, h->xn, vt_loc, D, L, D, D, D, L, G3C_EPI_BF16, nullptr, 0, st));  // V^T
         if (h->cp_size > 1) {
           // baseline mode (G3C_CP_MODE=nccl): one in-place all-gather of K and of V^T per layer on a side stream
@@ -497,7 +453,7 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
           G3C_CUDA(cudaEventRecord(h->ev_gathered, h->comm_stream));
           n += 2;
         }
-        TRY(proj_norm_rope(h->xn, s.wq, h->q, L, D, s.gq, h->rope, n));
+        K(CAT_GEMM, proj_norm_rope(h->xn, s.wq, h->q, L, D, s.gq, h->rope));
         if (h->cp_size > 1) G3C_CUDA(cudaStreamWaitEvent(st, h->ev_gathered, 0));
         K(CAT_ATTN_SELF, attn_fwd(h->q, h->k_all, h->vt_all, h->att, L, Lk_all, heads, D, D, D, L, attn_scale, st));
       }
@@ -509,9 +465,9 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
       const float* m = h->mods + (size_t)(i * 3 + 1) * 3 * D;
       const int C = c.context_dim, M = h->ctx_len;
       K(CAT_ELTWISE, ln_modulate(h->x, nullptr, m, m + D, h->xn, L, D, 1e-6f, st));
-      TRY(proj_norm_rope(ctx, s.wk, h->kc, M, C, s.gk, nullptr, n));
+      K(CAT_GEMM, proj_norm_rope(ctx, s.wk, h->kc, M, C, s.gk, nullptr));
       K(CAT_GEMM, gemm_bf16(s.wv, ctx, h->vtc, D, M, C, C, C, M, G3C_EPI_BF16, nullptr, 0, st));
-      TRY(proj_norm_rope(h->xn, s.wq, h->q, L, D, s.gq, nullptr, n));
+      K(CAT_GEMM, proj_norm_rope(h->xn, s.wq, h->q, L, D, s.gq, nullptr));
       K(CAT_ATTN_CROSS, attn_fwd(h->q, h->kc, h->vtc, h->att, L, M, heads, D, D, D, M, attn_scale, st));
       K(CAT_GEMM, gemm_bf16(h->att, s.wo, h->x, L, D, D, D, D, D, G3C_EPI_GATED_RESIDUAL_F32, m + 2 * D, 0, st));
     }
@@ -628,10 +584,6 @@ int g3c_dit_enable_cp(g3c_dit_t* h, const void* nccl_unique_id, int cp_rank, int
     h->comm = nullptr;
   }
   h->cp_p2p = nccl_unique_id == nullptr;  // NULL id: fused peer-memory mode (default); else NCCL all-gather mode
-  {
-    const char* e = getenv("G3C_CP_PUSH");
-    h->cp_push_sm = e && e[0] == 's';
-  }
   if (!h->cp_p2p) {
     if (!nccl().ok) {
       set_error("libnccl.so.2 could not be loaded");
@@ -836,9 +788,7 @@ int g3c_denoise_step(g3c_dit_t* h, const g3c_step_args* a, void* stream) {
     char* own = (char*)h->cfg_region;
     TRY(prof_mark(h, CAT_COMM, true, st));
     G3C_CUDA(cudaMemcpyAsync(peer + (size_t)slot * h->cfg_slot_bytes, mine, bytes, cudaMemcpyDeviceToDevice, st));
-    PeerDst pf;
-    pf.ptr[pf.n++] = peer + 2 * h->cfg_slot_bytes + (size_t)slot * 4;
-    k_cp_signal<<<1, 32, 0, st>>>(pf, seq);
+    k_cp_signal<<<1, 1, 0, st>>>((uint32_t*)(peer + 2 * h->cfg_slot_bytes) + slot, seq);
     k_wait_flag<<<1, 32, 0, st>>>((const uint32_t*)(own + 2 * h->cfg_slot_bytes) + slot, seq, peer_timeout_ns());
     G3C_CUDA(cudaGetLastError());
     TRY(prof_mark(h, CAT_COMM, false, st));

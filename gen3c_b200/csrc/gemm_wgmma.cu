@@ -30,8 +30,6 @@ struct GemmParams {
   const float* gate;   // [N] for EPI_GATED_RESIDUAL
   int num_m_blk, num_n_blk, num_k_blk;
   int super_n;         // n-blocks per super-column (L2 reuse of the B operand)
-  int n_peer;          // bf16 epilogues: additional destinations (peer GPUs), same offsets as D
-  void* peer[7];
   // EPI_NORM_ROPE_BF16: per-head (128 columns) RMSNorm gain [128], cos|sin table [M][128] (or NULL: no rotation), eps
   const float* nr_gamma;
   const float* nr_cs;
@@ -149,17 +147,8 @@ __device__ __forceinline__ void epilogue(const float (&acc)[BN / 2], const GemmP
             v1 = gelu_erf(v1);
           }
           __nv_bfloat16* dptr = reinterpret_cast<__nv_bfloat16*>(p.D) + (size_t)row * p.ldd + col;
-          if (pair) {
-            const uint32_t q = pack_bf16x2(v0, v1);
-            *reinterpret_cast<uint32_t*>(dptr) = q;
-            // fused all-gather: the same bytes go to the peers' copies over NVLink (posted writes)
-#pragma unroll
-            for (int pd = 0; pd < 7; ++pd)
-              if (pd < p.n_peer)
-                *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.peer[pd]) + (size_t)row * p.ldd + col) = q;
-          } else {
-            dptr[0] = __float2bfloat16_rn(v0);
-          }
+          if (pair) *reinterpret_cast<uint32_t*>(dptr) = pack_bf16x2(v0, v1);
+          else dptr[0] = __float2bfloat16_rn(v0);
         } else {
           float* dptr = reinterpret_cast<float*>(p.D) + (size_t)row * p.ldd + col;
           if constexpr (EPI == G3C_EPI_GATED_RESIDUAL_F32) {
@@ -308,19 +297,16 @@ static int dispatch_epi(int epi, const CUtensorMap& tmA, const CUtensorMap& tmB,
 
 // Host entry used by the engine and by the C ABI.
 int gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, int lda, int ldb, int ldd,
-              int epilogue, const float* gate, int block_n, cudaStream_t st, const PeerDst* peers,
-              const NormRope* norm_rope) {
+              int epilogue, const float* gate, int block_n, cudaStream_t st, const NormRope* norm_rope) {
   G3C_REQUIRE(A && B && D, "gemm: null operand");
   if (norm_rope) {
-    G3C_REQUIRE(epilogue == G3C_EPI_BF16 && N % 128 == 0 && norm_rope->gamma && (!peers || peers->n == 0),
-                "gemm: the RMSNorm/RoPE epilogue needs the bf16 epilogue, N %% 128 == 0, a gain vector and no peers");
+    G3C_REQUIRE(epilogue == G3C_EPI_BF16 && N % 128 == 0 && norm_rope->gamma,
+                "gemm: the RMSNorm/RoPE epilogue needs the bf16 epilogue, N %% 128 == 0 and a gain vector");
     G3C_REQUIRE((reinterpret_cast<uintptr_t>(norm_rope->gamma) & 15) == 0 &&
                     (reinterpret_cast<uintptr_t>(norm_rope->cs) & 15) == 0,
                 "gemm: RMSNorm gain / RoPE table must be 16-byte aligned");
     epilogue = EPI_NORM_ROPE_BF16;
   }
-  G3C_REQUIRE(!peers || peers->n == 0 || (epilogue == G3C_EPI_BF16 && N % 32 == 0 && peers->n <= 7),
-              "gemm: peer destinations need the bf16 epilogue, N %% 32 == 0 and at most 7 peers");
   G3C_REQUIRE(M > 0 && N > 0 && K > 0, "gemm: bad shape %dx%dx%d", M, N, K);
   G3C_REQUIRE(K % 8 == 0 && lda % 8 == 0 && ldb % 8 == 0, "gemm: K/lda/ldb must be multiples of 8");
   G3C_REQUIRE(lda >= K && ldb >= K && ldd >= N, "gemm: leading dimension smaller than extent");
@@ -360,8 +346,6 @@ int gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, int ld
   p.ldd = ldd;
   p.D = D;
   p.gate = gate;
-  p.n_peer = peers ? peers->n : 0;
-  for (int i = 0; i < 7; ++i) p.peer[i] = (peers && i < peers->n) ? peers->ptr[i] : nullptr;
   p.nr_gamma = norm_rope ? norm_rope->gamma : nullptr;
   p.nr_cs = norm_rope ? norm_rope->cs : nullptr;
   p.nr_eps = norm_rope ? norm_rope->eps : 0.0f;
@@ -387,7 +371,7 @@ extern "C" int g3c_gemm_bf16(const void* A, const void* B, void* D, int M, int N
                              int ldb, int ldd, int epilogue, const float* gate, int block_n,
                              void* stream) {
   return g3c::gemm_bf16(A, B, D, M, N, K, lda, ldb, ldd, epilogue, gate, block_n,
-                        (cudaStream_t)stream, nullptr);
+                        (cudaStream_t)stream);
 }
 
 extern "C" int g3c_gemm_norm_rope_bf16(const void* A, const void* B, void* D, int M, int N, int K, int lda, int ldb,
@@ -396,5 +380,5 @@ extern "C" int g3c_gemm_norm_rope_bf16(const void* A, const void* B, void* D, in
   nr.gamma = gamma;
   nr.cs = cos_sin;
   nr.eps = eps;
-  return g3c::gemm_bf16(A, B, D, M, N, K, lda, ldb, ldd, G3C_EPI_BF16, nullptr, 0, (cudaStream_t)stream, nullptr, &nr);
+  return g3c::gemm_bf16(A, B, D, M, N, K, lda, ldb, ldd, G3C_EPI_BF16, nullptr, 0, (cudaStream_t)stream, &nr);
 }

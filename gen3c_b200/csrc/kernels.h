@@ -4,13 +4,6 @@
 
 namespace g3c {
 
-// Extra destinations of a bf16 epilogue / of the RMSNorm-RoPE pass: the same tile is also stored at the same
-// offset of up to 7 peer buffers (NVLink peer memory) — the fused "compute -> all-gather" of context parallelism.
-struct PeerDst {
-  int n = 0;
-  void* ptr[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-};
-
 // Optional fused tail of a projection: per-head (128 columns) RMSNorm with gain `gamma` [128] and, when `cs` is given,
 // rotate-half RoPE with the cos|sin table `cs` [M][128] — applied to the fp32 accumulators in the GEMM epilogue.
 struct NormRope {
@@ -20,8 +13,7 @@ struct NormRope {
 };
 
 int gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, int lda, int ldb, int ldd,
-              int epilogue, const float* gate, int block_n, cudaStream_t st, const PeerDst* peers = nullptr,
-              const NormRope* norm_rope = nullptr);
+              int epilogue, const float* gate, int block_n, cudaStream_t st, const NormRope* norm_rope = nullptr);
 // Chunk-ordered attention for context parallelism: KV chunk c (= source rank) may only be read once
 // flags[c] >= seq (written with system scope by rank c after its K / V^T slices have landed here); chunks are
 // visited starting at `first` so that the local chunk overlaps the arrival of the remote ones.
@@ -47,7 +39,7 @@ struct PatchSrc {
 int ln_modulate(float* x, const __nv_bfloat16* pos, const float* shift, const float* scale,
                 __nv_bfloat16* y, int L, int D, float eps, cudaStream_t st);
 int rmsnorm_rope(__nv_bfloat16* qk, int ld, int L, int heads, const float* gamma, const float* cs,
-                 float eps, cudaStream_t st, const PeerDst* peers = nullptr);
+                 float eps, cudaStream_t st);
 int gemv(const __nv_bfloat16* W, const float* x, const float* add, float* y, int N, int K, int pre,
          int round_out, cudaStream_t st);
 int patchify(const PatchSrc& src, int T, int Hp, int Wp, int Kpad, __nv_bfloat16* out, cudaStream_t st);

@@ -15,8 +15,6 @@
 //                           4 x red.global.add.v4.f32 {r*w, g*w, b*w, w} per source pixel
 //   pass 3  k_normalise   : crop the 1-px ring, acc/w, fill, clamp, write planar outputs
 // HBM-bound by design: algorithmic traffic 44 B/px (SURVEY.md §8d).
-#include <cstdlib>
-
 #include "common.cuh"
 
 namespace g3c {
@@ -1252,15 +1250,10 @@ static int render_items(g3c_render* r, const float* points, const float* image, 
     } else {
       G3C_CUDA(cudaMemsetAsync(r->acc, 0, plane * 4 * sizeof(float) * n, st));
       if (want_depth) G3C_CUDA(cudaMemsetAsync(r->accz, 0, plane * sizeof(float) * n, st));
-      // G3C_SPLAT=ref: the round-1 one-pixel-per-thread kernel with the reference's exact weight arithmetic (A/B runs)
-      static int fast = -1;
-      if (fast < 0) {
-        const char* e = getenv("G3C_SPLAT");
-        fast = !(e && e[0] == 'r');
-      }
+      // 4 pixels per thread with 16-byte loads; frames with W % 4 != 0 or unaligned inputs take one pixel per thread
       const bool aligned = (W % 4 == 0) && ((reinterpret_cast<uintptr_t>(points) | reinterpret_cast<uintptr_t>(image) |
                                              reinterpret_cast<uintptr_t>(mask) | reinterpret_cast<uintptr_t>(flow_out)) % 16 == 0);
-      if (fast && aligned)
+      if (aligned)
         k_splat_points4<<<px_grid(HW / 4, n), 256, 0, st>>>(points, image, mask, w2c, K, map, i0, C, H, W, group, r->gmax,
                                                             r->acc, want_depth ? r->accz : nullptr, flow_out);
       else

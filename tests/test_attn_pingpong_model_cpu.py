@@ -16,8 +16,7 @@ The roles run under random interleavings.  The model checks what the hardware te
   * P.V(j) reads P_j, and P_j is packed (over P_{j-1}) only after P.V(j-1) has retired;
   * O is rescaled only after P.V(j-1) has retired, and the softmax reads S_j only after S_j has retired;
   * MMAs are issued only while the warpgroup holds the turn, and the turn strictly alternates 0, 1, 0, 1, ...
-mbarrier semantics: `wait(parity)` passes when the barrier's current phase parity differs from `parity`.
-tests/test_attn_pipeline_model_cpu.py models a different protocol (a single MMA issuer with several S buffers)."""
+mbarrier semantics: `wait(parity)` passes when the barrier's current phase parity differs from `parity`."""
 import random
 
 import pytest

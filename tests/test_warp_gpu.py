@@ -43,6 +43,27 @@ def test_forward_warp_matches_reference_golden(name, golden_dir):
     assert close_frac(d[same[:, 0]], g["depth"][same[:, 0]], 1e-3) > 0.999
 
 
+def test_forward_warp_width_not_multiple_of_4():
+    """A frame with W % 4 != 0 takes the one-pixel-per-thread splat kernel (k_splat_points), not the 4-pixel one."""
+    from gen3c_b200 import warp
+
+    c = cases.warp_case("R6")
+    depth, image = (np.ascontiguousarray(c[k][..., :126]) for k in ("depth", "image"))
+    pts = warp.unproject_points(cu(depth), cu(c["w2c_src"]), cu(c["K"]))
+    w, m, d, f = warp.forward_warp(cu(image), None, None, None, cu(c["w2c_tgt"]), cu(c["K"]), cu(c["K"]),
+                                   render_depth=True, world_points1=pts)
+    torch.cuda.synchronize()
+    w, m, d, f = (t.cpu().numpy() for t in (w, m, d, f))
+    wo, mo, do, fo = warp_oracle.forward_warp(image, None, pts.cpu().numpy(), c["w2c_tgt"], c["K"], render_depth=True)
+    np.testing.assert_allclose(f, fo, atol=2e-3)
+    assert (m != mo).mean() < 2e-3
+    same = (m == mo) & (mo > 0)
+    sel = np.broadcast_to(same, w.shape)
+    assert close_frac(w[sel], wo[sel], 2e-3) > 0.999
+    assert np.abs(w[sel] - wo[sel]).mean() < 1e-4
+    assert close_frac(d[same[:, 0]], do[same[:, 0]], 1e-3) > 0.999
+
+
 @pytest.mark.parametrize("name", ["R2", "R4", "R6"])
 def test_splat_indices_bit_exact(name, golden_dir):
     """Integer work: floor/ceil/clamp destination indices on the reference's own coordinates."""
