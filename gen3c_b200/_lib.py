@@ -84,6 +84,10 @@ SIGNATURES = {
     "g3c_render_cache_occlusion": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _I, _I, _P]),
     "g3c_gemm_bf16": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _I, _P]),
     "g3c_gemm_norm_rope_bf16": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _F, _P]),
+    "g3c_quantize_rows_fp8": (_I, [_P, _I, _I, _I, _P, _I, _P, _P]),
+    "g3c_gemm_fp8": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _I, _P]),
+    "g3c_gemm_norm_rope_fp8": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _F, _P]),
+    "g3c_ln_modulate_fp8": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _F, _P]),
     "g3c_attn_fwd": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _F, _P]),
     "g3c_attn_fwd_sbhd": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _F, _P]),
     "g3c_attn_set_trace": (_I, [_P]),
@@ -98,6 +102,7 @@ SIGNATURES = {
     "g3c_dit_cp_import": (_I, [_P, _P, _I]),
     "g3c_dit_cp_mode": (_I, [_P]),
     "g3c_dit_disable_cp": (_I, [_P]),
+    "g3c_dit_set_linear_fp8": (_I, [_P, _I]),
     "g3c_dit_enable_cfg_parallel": (_I, [_P, _I]),
     "g3c_dit_cfg_export": (_I, [_P, _P]),
     "g3c_dit_cfg_import": (_I, [_P, _P]),

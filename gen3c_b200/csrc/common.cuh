@@ -31,10 +31,11 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line);
     }                                 \
   } while (0)
 
-// Host: encode a tiled TMA descriptor (bf16, 128-byte swizzle).  dims/strides innermost first.
-// rank 2 or 3.  strides_bytes has rank-1 entries (stride of dim 1.., dim 0 is contiguous).
+// Host: encode a tiled TMA descriptor (128-byte swizzle) of bf16 elements, or of `dtype` (UINT8 for e4m3 codes).
+// dims/strides innermost first, rank 2 or 3.  strides_bytes has rank-1 entries (stride of dim 1.., dim 0 is contiguous).
 int make_tmap_bf16_sw128(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
-                         const uint64_t* strides_bytes, const uint32_t* box);
+                         const uint64_t* strides_bytes, const uint32_t* box,
+                         CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
 // Same for a 2-D fp32 tensor (box inner extent 32 floats = one 128-byte swizzle span).
 int make_tmap_f32_sw128(CUtensorMap* out, const void* base, const uint64_t* dims,
                         const uint64_t* strides_bytes, const uint32_t* box);

@@ -7,6 +7,10 @@
 //   unpatch : general_dit.py:348-357 "(p1 p2 t C)"
 //   t-embed : blocks.py:38-51,68-80 ; abs-pos normalise: position_embedding.py:220-233
 //   sampler : model/model_v2w.py:130-149,201-259 ; EDM Euler (diffusers 0.32.2, restated)
+#include <cuda_fp8.h>
+
+#include <type_traits>
+
 #include "kernels.h"
 
 namespace g3c {
@@ -27,14 +31,68 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
   return t;  // every thread of every warp holds the block total
 }
 
+__device__ __forceinline__ float block_max(float v, float* red) {
+  v = warp_max(v);
+  int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  __syncthreads();
+  if (lane == 0) red[w] = v;
+  __syncthreads();
+  int nw = (blockDim.x + 31) >> 5;
+  float t = lane < nw ? red[lane] : 0.0f;
+  return warp_max(t);
+}
+
+// ------------------------------------------------------------------------------------------------
+// e4m3 row quantisation (the fp8 Linear mode; DESIGN.md §3.1): for a row with amax = max |x|,
+//   inv = 448 / amax (IEEE division), code = e4m3_rn_satfinite(x * inv), scale = amax / 448;
+//   a zero row gets codes 0 and scale 1.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float e4m3_inv_scale(float amax) { return amax > 0.0f ? __fdiv_rn(448.0f, amax) : 0.0f; }
+__device__ __forceinline__ float e4m3_row_scale(float amax) { return amax > 0.0f ? __fdiv_rn(amax, 448.0f) : 1.0f; }
+// four codes, the first in the lowest byte
+__device__ __forceinline__ uint32_t e4m3x4(float a, float b, float c, float d, float inv) {
+  const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(__fmul_rn(a, inv), __fmul_rn(b, inv)), __NV_SATFINITE, __NV_E4M3);
+  const uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(__fmul_rn(c, inv), __fmul_rn(d, inv)), __NV_SATFINITE, __NV_E4M3);
+  return lo | (hi << 16);
+}
+
+// bf16 x [R, C] (ld) -> codes [R, C] (ldq) + scales [R]; one CTA per row, 8 elements per thread and step
+__global__ void __launch_bounds__(256)
+    k_quant_rows_e4m3(const __nv_bfloat16* __restrict__ x, int ld, int C, uint8_t* __restrict__ codes, int ldq,
+                      float* __restrict__ scales) {
+  __shared__ float red[32];
+  const __nv_bfloat16* xr = x + (size_t)blockIdx.x * ld;
+  float amax = 0.0f;
+  for (int i = threadIdx.x * 8; i < C; i += blockDim.x * 8) {
+    uint4 q = *reinterpret_cast<const uint4*>(xr + i);
+    const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&q);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) amax = fmaxf(amax, fmaxf(fabsf(__low2float(h[j])), fabsf(__high2float(h[j]))));
+  }
+  amax = block_max(amax, red);
+  const float inv = e4m3_inv_scale(amax);
+  uint8_t* cr = codes + (size_t)blockIdx.x * ldq;
+  for (int i = threadIdx.x * 8; i < C; i += blockDim.x * 8) {
+    uint4 q = *reinterpret_cast<const uint4*>(xr + i);
+    const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&q);
+    uint2 o;
+    o.x = e4m3x4(__low2float(h[0]), __high2float(h[0]), __low2float(h[1]), __high2float(h[1]), inv);
+    o.y = e4m3x4(__low2float(h[2]), __high2float(h[2]), __low2float(h[3]), __high2float(h[3]), inv);
+    *reinterpret_cast<uint2*>(cr + i) = o;
+  }
+  if (threadIdx.x == 0) scales[blockIdx.x] = e4m3_row_scale(amax);
+}
+
 // ------------------------------------------------------------------------------------------------
 // x (fp32 residual stream) [+= pos] ; y = LN(x) * (1 + scale) + shift   -> bf16
 // one CTA per token row, the row cached in shared memory between the two statistics passes
+// TOut = uint8_t: y is quantised to e4m3 codes from the fp32 row (never rounded to bf16) with the row scale in y_scale
 // ------------------------------------------------------------------------------------------------
+template <typename TOut>
 __global__ void __launch_bounds__(256)
     k_ln_modulate(float* __restrict__ x, const __nv_bfloat16* __restrict__ pos,
                   const float* __restrict__ shift, const float* __restrict__ scale,
-                  __nv_bfloat16* __restrict__ y, int D, float eps) {
+                  TOut* __restrict__ y, int D, float eps, float* __restrict__ y_scale) {
   extern __shared__ float row[];
   __shared__ float red[32];
   const size_t base = (size_t)blockIdx.x * D;
@@ -62,16 +120,37 @@ __global__ void __launch_bounds__(256)
     sq += (a * a + b * b) + (c * c + d * d);
   }
   const float rstd = rsqrtf(block_sum(sq, red) / (float)D + eps);
-  for (int i = threadIdx.x * 4; i < D; i += blockDim.x * 4) {
-    float4 v = *reinterpret_cast<const float4*>(row + i);
-    float4 sc = *reinterpret_cast<const float4*>(scale + i);
-    float4 sh = *reinterpret_cast<const float4*>(shift + i);
-    uint2 o;
-    o.x = pack_bf16x2(fmaf((v.x - mean) * rstd, 1.0f + sc.x, sh.x),
-                      fmaf((v.y - mean) * rstd, 1.0f + sc.y, sh.y));
-    o.y = pack_bf16x2(fmaf((v.z - mean) * rstd, 1.0f + sc.z, sh.z),
-                      fmaf((v.w - mean) * rstd, 1.0f + sc.w, sh.w));
-    *reinterpret_cast<uint2*>(y + base + i) = o;
+  if constexpr (std::is_same<TOut, __nv_bfloat16>::value) {
+    for (int i = threadIdx.x * 4; i < D; i += blockDim.x * 4) {
+      float4 v = *reinterpret_cast<const float4*>(row + i);
+      float4 sc = *reinterpret_cast<const float4*>(scale + i);
+      float4 sh = *reinterpret_cast<const float4*>(shift + i);
+      uint2 o;
+      o.x = pack_bf16x2(fmaf((v.x - mean) * rstd, 1.0f + sc.x, sh.x),
+                        fmaf((v.y - mean) * rstd, 1.0f + sc.y, sh.y));
+      o.y = pack_bf16x2(fmaf((v.z - mean) * rstd, 1.0f + sc.z, sh.z),
+                        fmaf((v.w - mean) * rstd, 1.0f + sc.w, sh.w));
+      *reinterpret_cast<uint2*>(y + base + i) = o;
+    }
+  } else {
+    // the modulated row replaces x in shared memory (each thread rewrites and rereads its own elements)
+    float amax = 0.0f;
+    for (int i = threadIdx.x * 4; i < D; i += blockDim.x * 4) {
+      float4 v = *reinterpret_cast<const float4*>(row + i);
+      float4 sc = *reinterpret_cast<const float4*>(scale + i);
+      float4 sh = *reinterpret_cast<const float4*>(shift + i);
+      v = make_float4(fmaf((v.x - mean) * rstd, 1.0f + sc.x, sh.x), fmaf((v.y - mean) * rstd, 1.0f + sc.y, sh.y),
+                      fmaf((v.z - mean) * rstd, 1.0f + sc.z, sh.z), fmaf((v.w - mean) * rstd, 1.0f + sc.w, sh.w));
+      *reinterpret_cast<float4*>(row + i) = v;
+      amax = fmaxf(amax, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
+    }
+    amax = block_max(amax, red);
+    const float inv = e4m3_inv_scale(amax);
+    for (int i = threadIdx.x * 4; i < D; i += blockDim.x * 4) {
+      float4 v = *reinterpret_cast<const float4*>(row + i);
+      *reinterpret_cast<uint32_t*>(y + base + i) = e4m3x4(v.x, v.y, v.z, v.w, inv);
+    }
+    if (threadIdx.x == 0) y_scale[blockIdx.x] = e4m3_row_scale(amax);
   }
 }
 
@@ -331,10 +410,38 @@ int ln_modulate(float* x, const __nv_bfloat16* pos, const float* shift, const fl
   G3C_REQUIRE(D % 4 == 0 && D * 4 <= 96 * 1024, "ln_modulate: D=%d unsupported", D);
   static bool configured = false;
   if (!configured) {
-    G3C_CUDA(cudaFuncSetAttribute(k_ln_modulate, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+    G3C_CUDA(cudaFuncSetAttribute(k_ln_modulate<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
     configured = true;
   }
-  k_ln_modulate<<<L, 256, D * sizeof(float), st>>>(x, pos, shift, scale, y, D, eps);
+  k_ln_modulate<__nv_bfloat16><<<L, 256, D * sizeof(float), st>>>(x, pos, shift, scale, y, D, eps, nullptr);
+  G3C_CUDA(cudaGetLastError());
+  return G3C_OK;
+}
+
+int ln_modulate_e4m3(float* x, const __nv_bfloat16* pos, const float* shift, const float* scale, uint8_t* y8,
+                     float* y_scale, int L, int D, float eps, cudaStream_t st) {
+  G3C_REQUIRE(D % 16 == 0 && D * 4 <= 96 * 1024, "ln_modulate_e4m3: D=%d unsupported", D);
+  static bool configured = false;
+  if (!configured) {
+    G3C_CUDA(cudaFuncSetAttribute(k_ln_modulate<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+    configured = true;
+  }
+  k_ln_modulate<uint8_t><<<L, 256, D * sizeof(float), st>>>(x, pos, shift, scale, y8, D, eps, y_scale);
+  G3C_CUDA(cudaGetLastError());
+  return G3C_OK;
+}
+
+int quant_rows_e4m3(const __nv_bfloat16* x, int ld, int R, int C, uint8_t* codes, int ldq, float* scales,
+                    cudaStream_t st) {
+  G3C_REQUIRE(x && codes && scales, "quantize_rows_fp8: null argument");
+  G3C_REQUIRE(R > 0 && C > 0 && C % 16 == 0, "quantize_rows_fp8: C=%d must be a positive multiple of 16 (R=%d)", C, R);
+  G3C_REQUIRE(ld >= C && ld % 8 == 0 && ldq >= C && ldq % 16 == 0,
+              "quantize_rows_fp8: leading dimensions ld=%d (multiple of 8) and ldq=%d (multiple of 16) must be >= C=%d",
+              ld, ldq, C);
+  G3C_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(codes) & 15) == 0 &&
+                  (reinterpret_cast<uintptr_t>(scales) & 15) == 0,
+              "quantize_rows_fp8: x, codes and scales must be 16-byte aligned");
+  k_quant_rows_e4m3<<<R, 256, 0, st>>>(x, ld, C, codes, ldq, scales);
   G3C_CUDA(cudaGetLastError());
   return G3C_OK;
 }
@@ -426,6 +533,21 @@ int g3c_ln_modulate(float* x, const void* pos_bf16, const float* shift, const fl
   G3C_REQUIRE(x && shift && scale && y_bf16 && L > 0, "ln_modulate: bad arguments");
   return g3c::ln_modulate(x, (const __nv_bfloat16*)pos_bf16, shift, scale, (__nv_bfloat16*)y_bf16, L, D,
                           eps, (cudaStream_t)stream);
+}
+
+int g3c_quantize_rows_fp8(const void* x_bf16, int ld, int R, int C, void* codes, int ldq, float* scales,
+                          void* stream) {
+  return g3c::quant_rows_e4m3((const __nv_bfloat16*)x_bf16, ld, R, C, (uint8_t*)codes, ldq, scales,
+                              (cudaStream_t)stream);
+}
+
+int g3c_ln_modulate_fp8(float* x, const void* pos_bf16, const float* shift, const float* scale, void* y_codes,
+                        float* y_scales, int L, int D, float eps, void* stream) {
+  G3C_REQUIRE(x && shift && scale && y_codes && y_scales && L > 0, "ln_modulate_fp8: bad arguments");
+  G3C_REQUIRE((reinterpret_cast<uintptr_t>(y_codes) & 15) == 0 && (reinterpret_cast<uintptr_t>(y_scales) & 15) == 0,
+              "ln_modulate_fp8: codes and scales must be 16-byte aligned");
+  return g3c::ln_modulate_e4m3(x, (const __nv_bfloat16*)pos_bf16, shift, scale, (uint8_t*)y_codes, y_scales, L, D, eps,
+                               (cudaStream_t)stream);
 }
 
 int g3c_rmsnorm_rope(void* qk_bf16, int ld, int L, int heads, const float* gamma, const float* cos_sin,

@@ -80,11 +80,19 @@ struct WTensor {
   int dtype = 0;
 };
 
+// engine-owned e4m3 copy of one Linear weight [N, K]: codes + per-output-channel scales [N]
+struct W8 {
+  uint8_t* codes = nullptr;
+  float* scale = nullptr;
+};
+
 struct SubBlock {
   const __nv_bfloat16 *wq = nullptr, *wk = nullptr, *wv = nullptr, *wo = nullptr;  // attention
   const float *gq = nullptr, *gk = nullptr;                                        // RMSNorm gamma (f32 copy)
   const __nv_bfloat16 *w1 = nullptr, *w2 = nullptr;                                // MLP
   const __nv_bfloat16 *ada1 = nullptr, *ada2 = nullptr;                            // adaLN-LoRA
+  // fp8 Linear mode: FA to_q/to_k/to_v/to_out, CA to_q/to_out (q8, o8), MLP layer1/layer2 (l1, l2)
+  W8 q8, k8, v8, o8, l1, l2;
 };
 
 }  // namespace g3c
@@ -102,6 +110,11 @@ struct g3c_dit {
   __nv_bfloat16* w_patch_pad = nullptr;  // [D, Kpad] owned
   float* gammas = nullptr;               // owned f32 copies of the RMSNorm weights
   int Kpatch = 0, Kpad = 0;
+  // fp8 Linear mode (g3c_dit_set_linear_fp8): e4m3 copies of the eight large Linears of every block, quantised by
+  // resolve() from the registered bf16 weights, in one allocation of w8_bytes
+  bool fp8 = false;
+  void* w8 = nullptr;
+  size_t w8_bytes = 0;
 
   // shape
   int T = 0, Hl = 0, Wl = 0, Hp = 0, Wp = 0, L = 0, ctx_len = 0;
@@ -133,6 +146,9 @@ struct g3c_dit {
   float *rope = nullptr, *yfin = nullptr, *mods = nullptr, *modf = nullptr, *vec_s = nullptr,
         *vec_emb = nullptr, *vec_h1 = nullptr, *vec_lora = nullptr, *vec_a = nullptr, *freqs = nullptr;
   __nv_bfloat16 *lat_xtilde = nullptr, *lat_xin = nullptr, *lat_oc = nullptr, *lat_ou = nullptr;
+  // fp8 Linear mode: e4m3 codes + row scales of the GEMM A operands (xn, att, hid)
+  uint8_t *xn8 = nullptr, *att8 = nullptr, *hid8 = nullptr;
+  float *xn8_s = nullptr, *att8_s = nullptr, *hid8_s = nullptr;
   bool tables_ready = false;
   // the B=1 modulation vectors depend on the timestep only: the second forward of a denoise step reuses them
   bool mods_valid = false;
@@ -216,6 +232,28 @@ static int prof_mark(g3c_dit* h, int cat, bool begin, cudaStream_t st) {
     ++n;                                \
   } while (0)
 
+static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// Layout of the fp8 weight copies inside h->w8: per block, the eight Linears in the order FA q, k, v, out, CA q, out,
+// MLP layer1, layer2, each as codes [N, K] then scales [N].  Returns the bytes; assigns the W8 pointers when blk is sized.
+static size_t fp8_layout(g3c_dit* h) {
+  const size_t D = h->cfg.model_channels, F = h->cfg.ffn_dim;
+  const size_t nk[8][2] = {{D, D}, {D, D}, {D, D}, {D, D}, {D, D}, {D, D}, {F, D}, {D, F}};
+  size_t off = 0;
+  for (int i = 0; i < h->cfg.num_blocks; ++i) {
+    for (int j = 0; j < 8; ++j) {
+      if (h->w8 && (int)h->blk.size() == h->cfg.num_blocks) {
+        SubBlock &fa = h->blk[i][0], &ca = h->blk[i][1], &mlp = h->blk[i][2];
+        W8* dst[8] = {&fa.q8, &fa.k8, &fa.v8, &fa.o8, &ca.q8, &ca.o8, &mlp.l1, &mlp.l2};
+        dst[j]->codes = (uint8_t*)h->w8 + off;
+        dst[j]->scale = (float*)((char*)h->w8 + off + align_up(nk[j][0] * nk[j][1], 1024));
+      }
+      off += align_up(nk[j][0] * nk[j][1], 1024) + align_up(nk[j][0] * 4, 1024);
+    }
+  }
+  return off;
+}
+
 static int resolve(g3c_dit* h, cudaStream_t st) {
   if (h->resolved) return G3C_OK;
   const g3c_dit_config& c = h->cfg;
@@ -268,11 +306,21 @@ static int resolve(g3c_dit* h, cudaStream_t st) {
       }
     }
   }
+  if (h->fp8) {
+    fp8_layout(h);
+    // (re)quantise every fp8 Linear from the registered weights: reached after g3c_dit_load and after enabling the mode
+    for (int i = 0; i < c.num_blocks; ++i) {
+      const SubBlock &fa = h->blk[i][0], &ca = h->blk[i][1], &mlp = h->blk[i][2];
+      const struct { const __nv_bfloat16* w; const W8& q; int64_t n, k; } lin[8] = {
+          {fa.wq, fa.q8, D, D}, {fa.wk, fa.k8, D, D}, {fa.wv, fa.v8, D, D}, {fa.wo, fa.o8, D, D},
+          {ca.wq, ca.q8, D, D}, {ca.wo, ca.o8, D, D}, {mlp.w1, mlp.l1, F, D}, {mlp.w2, mlp.l2, D, F}};
+      for (const auto& l : lin)
+        TRY(quant_rows_e4m3(l.w, (int)l.k, (int)l.n, (int)l.k, l.q.codes, (int)l.k, l.q.scale, st));
+    }
+  }
   h->resolved = true;
   return G3C_OK;
 }
-
-static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 // Publish "my output of step `seq` has landed" in the CFG partner's flag.  Launched after the copy into the partner's
 // memory on the same stream (complete when this kernel starts); release at system scope.
@@ -359,6 +407,25 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
     nr.eps = 1e-6f;
     return gemm_bf16(a, w, out, M, D, Kin, Kin, Kin, D, G3C_EPI_BF16, nullptr, 0, st, &nr);
   };
+  // fp8 Linear mode (h->fp8): the eight large Linears of a block read e4m3 codes of their activation rows (xn8 from the
+  // fused LN-modulate, att8 / hid8 from a quantisation pass) and the engine's e4m3 weight copies; the GEMM dequantises
+  // with both row scales before its epilogue.  K and V^T stay bf16, so the context-parallel exchange is unchanged.
+  const bool f8 = h->fp8;
+  auto ln_mod = [&](const __nv_bfloat16* pos, const float* m) {
+    return f8 ? ln_modulate_e4m3(h->x, pos, m, m + D, h->xn8, h->xn8_s, L, D, 1e-6f, st)
+              : ln_modulate(h->x, pos, m, m + D, h->xn, L, D, 1e-6f, st);
+  };
+  auto proj8_norm_rope = [&](const W8& w, __nv_bfloat16* out, const float* gamma, const float* cs) {
+    NormRope nr;
+    nr.gamma = gamma;
+    nr.cs = cs;
+    nr.eps = 1e-6f;
+    return gemm_fp8(h->xn8, h->xn8_s, w.codes, w.scale, out, L, D, D, D, D, D, G3C_EPI_BF16, nullptr, 0, st, &nr);
+  };
+  // x += gate * (a8 . w^T), a8 = codes [L, Kin] of att (Kin = D) or hid (Kin = F)
+  auto out8 = [&](const uint8_t* a8, const float* sa, const W8& w, int Kin, const float* gate) {
+    return gemm_fp8(a8, sa, w.codes, w.scale, h->x, L, D, Kin, Kin, Kin, D, G3C_EPI_GATED_RESIDUAL_F32, gate, 0, st);
+  };
   int n = 0;
 
   // ---- input assembly + patch embedding (general_dit_video_conditioned.py:112-118,
@@ -398,7 +465,7 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
     {
       const SubBlock& s = h->blk[i][0];
       const float* m = h->mods + (size_t)(i * 3 + 0) * 3 * D;
-      K(CAT_ELTWISE, ln_modulate(h->x, h->pos, m, m + D, h->xn, L, D, 1e-6f, st));   // + abs-pos add
+      K(CAT_ELTWISE, ln_mod(h->pos, m));   // + abs-pos add
       if (h->cp_size > 1 && h->cp_p2p) {
         // all-gather through peer memory: every rank produces its K / V^T slice locally, then the copy engines push
         // it into every peer's buffer on a side stream and raise a flag there, while this stream already runs the Q
@@ -415,8 +482,13 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
         __nv_bfloat16* vb = (__nv_bfloat16*)(reg + h->off_vt[set]);
         __nv_bfloat16* kl = kb + (size_t)me * L * D;
         __nv_bfloat16* vl = vb + (size_t)me * L * D;
-        K(CAT_GEMM, proj_norm_rope(h->xn, s.wk, kl, L, D, s.gk, h->rope));
-        K(CAT_GEMM, gemm_bf16(s.wv, h->xn, vl, D, L, D, D, D, L, G3C_EPI_BF16, nullptr, 0, st));  // V^T
+        if (f8) {
+          K(CAT_GEMM, proj8_norm_rope(s.k8, kl, s.gk, h->rope));
+          K(CAT_GEMM, gemm_fp8(s.v8.codes, s.v8.scale, h->xn8, h->xn8_s, vl, D, L, D, D, D, L, G3C_EPI_BF16, nullptr, 0, st));
+        } else {
+          K(CAT_GEMM, proj_norm_rope(h->xn, s.wk, kl, L, D, s.gk, h->rope));
+          K(CAT_GEMM, gemm_bf16(s.wv, h->xn, vl, D, L, D, D, D, L, G3C_EPI_BF16, nullptr, 0, st));  // V^T
+        }
         G3C_CUDA(cudaEventRecord(h->ev_kv, st));
         G3C_CUDA(cudaStreamWaitEvent(h->comm_stream, h->ev_kv, 0));
         uint32_t* slot = h->seq_ring + (seq % g3c_dit::kSeqRing);
@@ -431,7 +503,8 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
           G3C_CUDA(cudaMemcpyAsync(pb + h->off_flags + (size_t)(set * 8 + me) * 4, slot, 4, cudaMemcpyHostToDevice,
                                    h->comm_stream));
         }
-        K(CAT_GEMM, proj_norm_rope(h->xn, s.wq, h->q, L, D, s.gq, h->rope));
+        if (f8) K(CAT_GEMM, proj8_norm_rope(s.q8, h->q, s.gq, h->rope));
+        else K(CAT_GEMM, proj_norm_rope(h->xn, s.wq, h->q, L, D, s.gq, h->rope));
         ChunkGate gate;
         gate.flags = (const uint32_t*)(reg + h->off_flags) + set * 8;
         gate.seq = seq;
@@ -440,8 +513,14 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
         h->wait_cta_launches = (double)((L + ATT_ROWS_PER_CTA - 1) / ATT_ROWS_PER_CTA) * heads;  // CTAs of one gated launch
         K(CAT_ATTN_SELF, attn_fwd(h->q, kb, vb, h->att, L, Lk_all, heads, D, D, D, L, attn_scale, st, &gate));
       } else {
-        K(CAT_GEMM, proj_norm_rope(h->xn, s.wk, k_loc, L, D, s.gk, h->rope));
-        K(CAT_GEMM, gemm_bf16(s.wv, h->xn, vt_loc, D, L, D, D, D, L, G3C_EPI_BF16, nullptr, 0, st));  // V^T
+        if (f8) {
+          K(CAT_GEMM, proj8_norm_rope(s.k8, k_loc, s.gk, h->rope));
+          K(CAT_GEMM, gemm_fp8(s.v8.codes, s.v8.scale, h->xn8, h->xn8_s, vt_loc, D, L, D, D, D, L, G3C_EPI_BF16, nullptr,
+                               0, st));
+        } else {
+          K(CAT_GEMM, proj_norm_rope(h->xn, s.wk, k_loc, L, D, s.gk, h->rope));
+          K(CAT_GEMM, gemm_bf16(s.wv, h->xn, vt_loc, D, L, D, D, D, L, G3C_EPI_BF16, nullptr, 0, st));  // V^T
+        }
         if (h->cp_size > 1) {
           // baseline mode (G3C_CP_MODE=nccl): one in-place all-gather of K and of V^T per layer on a side stream
           G3C_CUDA(cudaEventRecord(h->ev_kv, st));
@@ -453,31 +532,50 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
           G3C_CUDA(cudaEventRecord(h->ev_gathered, h->comm_stream));
           n += 2;
         }
-        K(CAT_GEMM, proj_norm_rope(h->xn, s.wq, h->q, L, D, s.gq, h->rope));
+        if (f8) K(CAT_GEMM, proj8_norm_rope(s.q8, h->q, s.gq, h->rope));
+        else K(CAT_GEMM, proj_norm_rope(h->xn, s.wq, h->q, L, D, s.gq, h->rope));
         if (h->cp_size > 1) G3C_CUDA(cudaStreamWaitEvent(st, h->ev_gathered, 0));
         K(CAT_ATTN_SELF, attn_fwd(h->q, h->k_all, h->vt_all, h->att, L, Lk_all, heads, D, D, D, L, attn_scale, st));
       }
-      K(CAT_GEMM, gemm_bf16(h->att, s.wo, h->x, L, D, D, D, D, D, G3C_EPI_GATED_RESIDUAL_F32, m + 2 * D, 0, st));
+      if (f8) {
+        K(CAT_ELTWISE, quant_rows_e4m3(h->att, D, L, D, h->att8, D, h->att8_s, st));
+        K(CAT_GEMM, out8(h->att8, h->att8_s, s.o8, D, m + 2 * D));
+      } else {
+        K(CAT_GEMM, gemm_bf16(h->att, s.wo, h->x, L, D, D, D, D, D, G3C_EPI_GATED_RESIDUAL_F32, m + 2 * D, 0, st));
+      }
     }
     // ---------------- CA: cross-attention to the T5 context (blocks.py:464-471)
     {
       const SubBlock& s = h->blk[i][1];
       const float* m = h->mods + (size_t)(i * 3 + 1) * 3 * D;
       const int C = c.context_dim, M = h->ctx_len;
-      K(CAT_ELTWISE, ln_modulate(h->x, nullptr, m, m + D, h->xn, L, D, 1e-6f, st));
+      K(CAT_ELTWISE, ln_mod(nullptr, m));
       K(CAT_GEMM, proj_norm_rope(ctx, s.wk, h->kc, M, C, s.gk, nullptr));
       K(CAT_GEMM, gemm_bf16(s.wv, ctx, h->vtc, D, M, C, C, C, M, G3C_EPI_BF16, nullptr, 0, st));
-      K(CAT_GEMM, proj_norm_rope(h->xn, s.wq, h->q, L, D, s.gq, nullptr));
+      if (f8) K(CAT_GEMM, proj8_norm_rope(s.q8, h->q, s.gq, nullptr));
+      else K(CAT_GEMM, proj_norm_rope(h->xn, s.wq, h->q, L, D, s.gq, nullptr));
       K(CAT_ATTN_CROSS, attn_fwd(h->q, h->kc, h->vtc, h->att, L, M, heads, D, D, D, M, attn_scale, st));
-      K(CAT_GEMM, gemm_bf16(h->att, s.wo, h->x, L, D, D, D, D, D, G3C_EPI_GATED_RESIDUAL_F32, m + 2 * D, 0, st));
+      if (f8) {
+        K(CAT_ELTWISE, quant_rows_e4m3(h->att, D, L, D, h->att8, D, h->att8_s, st));
+        K(CAT_GEMM, out8(h->att8, h->att8_s, s.o8, D, m + 2 * D));
+      } else {
+        K(CAT_GEMM, gemm_bf16(h->att, s.wo, h->x, L, D, D, D, D, D, G3C_EPI_GATED_RESIDUAL_F32, m + 2 * D, 0, st));
+      }
     }
     // ---------------- MLP (attention.py:91-102)
     {
       const SubBlock& s = h->blk[i][2];
       const float* m = h->mods + (size_t)(i * 3 + 2) * 3 * D;
-      K(CAT_ELTWISE, ln_modulate(h->x, nullptr, m, m + D, h->xn, L, D, 1e-6f, st));
-      K(CAT_GEMM, gemm_bf16(h->xn, s.w1, h->hid, L, F, D, D, D, F, G3C_EPI_GELU_BF16, nullptr, 0, st));
-      K(CAT_GEMM, gemm_bf16(h->hid, s.w2, h->x, L, D, F, F, F, D, G3C_EPI_GATED_RESIDUAL_F32, m + 2 * D, 0, st));
+      K(CAT_ELTWISE, ln_mod(nullptr, m));
+      if (f8) {
+        K(CAT_GEMM, gemm_fp8(h->xn8, h->xn8_s, s.l1.codes, s.l1.scale, h->hid, L, F, D, D, D, F, G3C_EPI_GELU_BF16,
+                             nullptr, 0, st));
+        K(CAT_ELTWISE, quant_rows_e4m3(h->hid, F, L, F, h->hid8, F, h->hid8_s, st));
+        K(CAT_GEMM, out8(h->hid8, h->hid8_s, s.l2, F, m + 2 * D));
+      } else {
+        K(CAT_GEMM, gemm_bf16(h->xn, s.w1, h->hid, L, F, D, D, D, F, G3C_EPI_GELU_BF16, nullptr, 0, st));
+        K(CAT_GEMM, gemm_bf16(h->hid, s.w2, h->x, L, D, F, F, F, D, G3C_EPI_GATED_RESIDUAL_F32, m + 2 * D, 0, st));
+      }
     }
   }
   // ---- final layer + unpatchify (blocks.py:222-242, general_dit.py:328-358)
@@ -541,6 +639,7 @@ int g3c_dit_destroy(g3c_dit_t* h) {
   free_ws(h);
   if (h->w_patch_pad) cudaFree(h->w_patch_pad);
   if (h->gammas) cudaFree(h->gammas);
+  if (h->w8) cudaFree(h->w8);
   if (h->comm && nccl().ok) nccl().CommDestroy(h->comm);
   if (h->comm_stream) cudaStreamDestroy(h->comm_stream);
   if (h->seq_ring) cudaFreeHost(h->seq_ring);
@@ -682,6 +781,14 @@ int g3c_dit_set_shape(g3c_dit_t* h, int T_local, int H_latent, int W_latent, int
       {(void**)&h->lat_xtilde, lat * 2},         {(void**)&h->lat_xin, lat * 2},
       {(void**)&h->lat_oc, lat * 2},             {(void**)&h->lat_ou, lat * 2},
   };
+  if (h->fp8) {
+    items.push_back({(void**)&h->xn8, (size_t)L * D});
+    items.push_back({(void**)&h->att8, (size_t)L * D});
+    items.push_back({(void**)&h->hid8, (size_t)L * F});
+    items.push_back({(void**)&h->xn8_s, (size_t)L * 4});
+    items.push_back({(void**)&h->att8_s, (size_t)L * 4});
+    items.push_back({(void**)&h->hid8_s, (size_t)L * 4});
+  }
   size_t total = 0;
   for (auto& it : items) total += align_up(it.bytes, 1024);
   cudaError_t e = cudaMalloc(&h->ws, total);
@@ -804,6 +911,33 @@ int g3c_denoise_step(g3c_dit_t* h, const g3c_step_args* a, void* stream) {
   return G3C_OK;
 }
 
+int g3c_dit_set_linear_fp8(g3c_dit_t* h, int on) {
+  G3C_REQUIRE(h, "set_linear_fp8: null handle");
+  G3C_REQUIRE(h->cfg.ffn_dim % 16 == 0, "set_linear_fp8: ffn_dim=%d must be a multiple of 16", h->cfg.ffn_dim);
+  if ((on != 0) == h->fp8) return G3C_OK;
+  free_ws(h);  // the fp8 activation buffers come and go with the shape's workspace
+  if (on) {
+    const size_t bytes = fp8_layout(h);
+    cudaError_t e = cudaMalloc(&h->w8, bytes);
+    if (e != cudaSuccess) {
+      h->w8 = nullptr;
+      set_error("set_linear_fp8: cudaMalloc of %zu bytes of e4m3 weights failed: %s", bytes, cudaGetErrorString(e));
+      return G3C_ENOMEM;
+    }
+    h->w8_bytes = bytes;
+  } else {
+    G3C_CUDA(cudaDeviceSynchronize());  // forwards still queued may read the copies
+    G3C_CUDA(cudaFree(h->w8));
+    h->w8 = nullptr;
+    h->w8_bytes = 0;
+    for (auto& b : h->blk)
+      for (auto& sb : b) sb.q8 = sb.k8 = sb.v8 = sb.o8 = sb.l1 = sb.l2 = W8();
+  }
+  h->fp8 = on != 0;
+  h->resolved = false;  // resolve() quantises the weights into the new copies
+  return G3C_OK;
+}
+
 int g3c_dit_enable_cfg_parallel(g3c_dit_t* h, int role) {
   G3C_REQUIRE(h && role <= 1, "enable_cfg_parallel: role must be 0 (cond), 1 (uncond) or negative (off)");
   h->cfg_role = role < 0 ? -1 : role;
@@ -870,7 +1004,7 @@ int g3c_dit_profile_read(g3c_dit_t* h, float* ms_by_category, int* launches_by_c
   return G3C_OK;
 }
 
-int64_t g3c_dit_workspace_bytes(const g3c_dit_t* h) { return h ? (int64_t)h->ws_bytes : 0; }
+int64_t g3c_dit_workspace_bytes(const g3c_dit_t* h) { return h ? (int64_t)(h->ws_bytes + h->w8_bytes) : 0; }
 int g3c_dit_last_launch_count(const g3c_dit_t* h) { return h ? h->launches : 0; }
 
 }  // extern "C"

@@ -14,6 +14,13 @@ struct NormRope {
 
 int gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, int lda, int ldb, int ldd,
               int epilogue, const float* gate, int block_n, cudaStream_t st, const NormRope* norm_rope = nullptr);
+// Same GEMM on e4m3 row-quantised operands: D = (A8 . B8^T) * scale_a[m] * scale_b[n], then the epilogue.
+int gemm_fp8(const void* A8, const float* scale_a, const void* B8, const float* scale_b, void* D, int M, int N, int K,
+             int lda, int ldb, int ldd, int epilogue, const float* gate, int block_n, cudaStream_t st,
+             const NormRope* norm_rope = nullptr);
+// Row quantiser: bf16 x [R, C] (ld) -> e4m3 codes [R, C] (ldq) + fp32 row scales [R] (amax / 448; 1 for a zero row).
+int quant_rows_e4m3(const __nv_bfloat16* x, int ld, int R, int C, uint8_t* codes, int ldq, float* scales,
+                    cudaStream_t st);
 // Chunk-ordered attention for context parallelism: KV chunk c (= source rank) may only be read once
 // flags[c] >= seq (written with system scope by rank c after its K / V^T slices have landed here); chunks are
 // visited starting at `first` so that the local chunk overlaps the arrival of the remote ones.
@@ -38,6 +45,9 @@ struct PatchSrc {
 
 int ln_modulate(float* x, const __nv_bfloat16* pos, const float* shift, const float* scale,
                 __nv_bfloat16* y, int L, int D, float eps, cudaStream_t st);
+// Same, the modulated row quantised straight from fp32: e4m3 codes y8 [L, D] + row scales y_scale [L].
+int ln_modulate_e4m3(float* x, const __nv_bfloat16* pos, const float* shift, const float* scale, uint8_t* y8,
+                     float* y_scale, int L, int D, float eps, cudaStream_t st);
 int rmsnorm_rope(__nv_bfloat16* qk, int ld, int L, int heads, const float* gamma, const float* cs,
                  float eps, cudaStream_t st);
 int gemv(const __nv_bfloat16* W, const float* x, const float* add, float* y, int N, int K, int pre,

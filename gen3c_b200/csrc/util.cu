@@ -42,7 +42,7 @@ static PFN_encodeTiled get_encode() {
 }
 
 int make_tmap_bf16_sw128(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
-                         const uint64_t* strides_bytes, const uint32_t* box) {
+                         const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapDataType dtype) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) {
     set_error("cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
@@ -72,7 +72,7 @@ int make_tmap_bf16_sw128(CUtensorMap* out, const void* base, int rank, const uin
       return G3C_EINVAL;
     }
   }
-  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base),
+  CUresult r = enc(out, dtype, (cuuint32_t)rank, const_cast<void*>(base),
                    gdims, gstr, gbox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);

@@ -4,7 +4,8 @@ engine in libgen3c_b200.so.
 Drop-in at the reference's network seam (SURVEY.md §8b-2): same constructor keywords, same
 ``state_dict`` key layout (so ``checkpoints/Gen3C-Cosmos-7B/model.pt`` loads unchanged under the
 ``net.`` prefix), same ``forward`` keyword arguments, ``enable_context_parallel`` /
-``disable_context_parallel`` / ``is_context_parallel_enabled``.
+``disable_context_parallel`` / ``is_context_parallel_enabled``.  Opt-in extension: ``enable_fp8_linear`` /
+``disable_fp8_linear`` / ``is_fp8_linear_enabled`` (e4m3 Linear layers, DESIGN.md §3.1).
 reference: cosmos_predict1/diffusion/networks/general_dit_video_conditioned.py:30-217,
            cosmos_predict1/diffusion/networks/general_dit.py:57-569
 """
@@ -96,6 +97,7 @@ class VideoExtendGeneralDIT(nn.Module):
         self.patch_spatial, self.patch_temporal = patch_spatial, patch_temporal
         self.cp_group = None
         self.cfg_group = None
+        self._fp8_linear = False
         self._handle = None
         self._registered_ptrs = None
         self._shape_key = None
@@ -257,6 +259,32 @@ class VideoExtendGeneralDIT(nn.Module):
         for g in (self.cp_group, self.cfg_group):
             if g is not None:
                 dist.barrier(group=g)
+
+    # ------------------------------------------------------------------------------------------
+    # FP8 Linear mode (extension; DESIGN.md §3.1)
+    # ------------------------------------------------------------------------------------------
+    @property
+    def is_fp8_linear_enabled(self) -> bool:
+        return self._fp8_linear
+
+    def enable_fp8_linear(self):
+        """Run the eight large Linears of every block (self-attention to_q/to_k/to_v/to_out, cross-attention to_q/to_out,
+        MLP layer1/layer2) on e4m3 codes with per-row scales: weights per output channel, activations per token.  The
+        engine keeps its own e4m3 copy of those weights (6.6 GB for the 7B net), re-quantised after every weight update.
+        The state_dict is unchanged."""
+        self._set_linear_fp8(True)
+
+    def disable_fp8_linear(self):
+        """Back to the bf16 forward; frees the e4m3 weight copies and activation buffers."""
+        self._set_linear_fp8(False)
+
+    def _set_linear_fp8(self, on: bool):
+        if on == self._fp8_linear:
+            return
+        self._teardown_barrier()  # the engine frees the shape's workspace, peer-mapped regions included
+        _lib.check(_lib.load().g3c_dit_set_linear_fp8(self._engine(), 1 if on else 0), "g3c_dit_set_linear_fp8")
+        self._fp8_linear = on
+        self._shape_key = None
 
     # ------------------------------------------------------------------------------------------
     # classifier-free-guidance parallelism (extension; SURVEY.md §8e "CFG x CP hybrid")

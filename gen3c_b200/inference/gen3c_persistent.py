@@ -90,6 +90,8 @@ class Gen3cPersistentModel:
                 synthetic=getattr(args, "synthetic", False))
         if process_group is not None:
             pipeline.model.net.enable_context_parallel(process_group)
+        if getattr(args, "fp8_linear", False):
+            pipeline.model.net.enable_fp8_linear()
         self.args = args
         self.frame_buffer_max = pipeline.model.frame_buffer_max
         self.generator = torch.Generator(device=device).manual_seed(args.seed)

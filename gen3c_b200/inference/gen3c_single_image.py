@@ -175,6 +175,8 @@ def demo(args, depth_predictor: Optional[Callable] = None, pipeline: Optional[Ge
             depth_predictor = load_moge(device)
     if process_group is not None:
         pipeline.model.net.enable_context_parallel(process_group)
+    if getattr(args, "fp8_linear", False):
+        pipeline.model.net.enable_fp8_linear()
 
     if args.batch_input_path:
         import json

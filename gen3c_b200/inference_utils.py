@@ -55,6 +55,9 @@ def add_common_arguments(parser: argparse.ArgumentParser) -> None:
                        ("--disable_prompt_encoder",
                         "Disable prompt encoder to save memory, returns dummy embeddings instead")):
         a(flag, action="store_true", help=text)
+    # not in the reference: an opt-in of this implementation
+    a("--fp8_linear", action="store_true",
+      help="Run the DiT's large Linear layers on FP8 (e4m3) tensor cores with per-row scales (off by default)")
 
 
 _IncompatibleKeys = namedtuple("IncompatibleKeys", ["missing_keys", "unexpected_keys", "incorrect_shapes"])

@@ -64,6 +64,94 @@ def gemm_norm_rope(a: torch.Tensor, b: torch.Tensor, gamma: torch.Tensor, cos_si
     return out
 
 
+def _rows_ld(t: torch.Tensor, dtype, name: str) -> int:
+    """Leading dimension of a 2-D CUDA tensor with contiguous rows; ValueError unless the fp8 kernels can read it."""
+    if not t.is_cuda or t.dtype != dtype:
+        raise ValueError(f"{name} must be a CUDA tensor of dtype {dtype}, got {t.dtype} on {t.device}")
+    if t.dim() != 2 or t.shape[0] < 1 or t.shape[1] < 1:
+        raise ValueError(f"{name} must be a non-empty 2-D tensor, got shape {tuple(t.shape)}")
+    if t.stride(1) != 1:
+        raise ValueError(f"the rows of {name} must be contiguous, got strides {t.stride()}")
+    if t.data_ptr() % 16 != 0:
+        raise ValueError(f"{name} must start on a 16-byte boundary")
+    return t.stride(0) if t.shape[0] > 1 else t.shape[1]
+
+
+def quantize_rows_fp8(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """Per-row e4m3 quantisation of bf16 x [R, C] (rows contiguous, any row stride that is a multiple of 8; C a
+    multiple of 16): codes [R, C] torch.float8_e4m3fn = e4m3_rn_satfinite(x * (448 / amax_r)), scales [R] float32 =
+    amax_r / 448 (1 for an all-zero row), so x ~= codes * scales[:, None]."""
+    ld = _rows_ld(x, torch.bfloat16, "x")
+    R, Cn = x.shape
+    if Cn % 16 != 0 or ld % 8 != 0:
+        raise ValueError(f"x: columns ({Cn}) must be a multiple of 16 and the row stride ({ld}) of 8")
+    codes = torch.empty((R, Cn), device=x.device, dtype=torch.float8_e4m3fn)
+    scales = torch.empty(R, device=x.device, dtype=torch.float32)
+    lib = _lib.load()
+    with torch.cuda.device(x.device):
+        _lib.check(lib.g3c_quantize_rows_fp8(x.data_ptr(), ld, R, Cn, codes.data_ptr(), Cn, scales.data_ptr(),
+                                             _lib.stream_ptr()), "g3c_quantize_rows_fp8")
+    return codes, scales
+
+
+def _fp8_operands(a, scale_a, b, scale_b):
+    lda, ldb = _rows_ld(a, torch.float8_e4m3fn, "a"), _rows_ld(b, torch.float8_e4m3fn, "b")
+    M, K = a.shape
+    N, K2 = b.shape
+    if K != K2:
+        raise ValueError(f"inner dimensions differ: a {tuple(a.shape)}, b {tuple(b.shape)}")
+    for t, n, want in ((scale_a, "scale_a", M), (scale_b, "scale_b", N)):
+        _chk(t, torch.float32, n)
+        if t.numel() != want or t.data_ptr() % 16 != 0:
+            raise ValueError(f"{n} must hold {want} float32 values and start on a 16-byte boundary")
+    if K % 16 != 0 or lda % 16 != 0 or ldb % 16 != 0:
+        raise ValueError(f"K ({K}) and the row strides of a ({lda}) and b ({ldb}) must be multiples of 16")
+    return M, N, K, lda, ldb
+
+
+def gemm_fp8(a: torch.Tensor, scale_a: torch.Tensor, b: torch.Tensor, scale_b: torch.Tensor, epilogue: int = EPI_BF16,
+             out: Optional[torch.Tensor] = None, gate: Optional[torch.Tensor] = None, block_n: int = 0) -> torch.Tensor:
+    """out[M,N] = epilogue((a[M,K] @ b[N,K]^T) * scale_a[:, None] * scale_b[None, :]) on the fp8 wgmma: a, b
+    torch.float8_e4m3fn codes (e.g. from quantize_rows_fp8), fp32 accumulation; epilogues as in `gemm`."""
+    M, N, K, lda, ldb = _fp8_operands(a, scale_a, b, scale_b)
+    odt = torch.bfloat16 if epilogue in (EPI_BF16, EPI_GELU_BF16) else torch.float32
+    if out is None:
+        if epilogue == EPI_GATED_RESIDUAL_F32:
+            raise ValueError("gated-residual epilogue accumulates into `out`")
+        out = torch.empty((M, N), device=a.device, dtype=odt)
+    _chk(out, odt, "out")
+    if tuple(out.shape) != (M, N):
+        raise ValueError(f"out must have shape {(M, N)}, got {tuple(out.shape)}")
+    if gate is not None:
+        _chk(gate, torch.float32, "gate")
+    lib = _lib.load()
+    with torch.cuda.device(a.device):
+        _lib.check(lib.g3c_gemm_fp8(a.data_ptr(), scale_a.data_ptr(), b.data_ptr(), scale_b.data_ptr(), out.data_ptr(),
+                                    M, N, K, lda, ldb, N, epilogue, _lib.ptr(gate), block_n, _lib.stream_ptr()),
+                   "g3c_gemm_fp8")
+    return out
+
+
+def gemm_norm_rope_fp8(a: torch.Tensor, scale_a: torch.Tensor, b: torch.Tensor, scale_b: torch.Tensor,
+                       gamma: torch.Tensor, cos_sin: Optional[torch.Tensor] = None, eps: float = 1e-6) -> torch.Tensor:
+    """`gemm_norm_rope` on e4m3 operands: the RMSNorm sees the dequantised accumulators."""
+    M, N, K, lda, ldb = _fp8_operands(a, scale_a, b, scale_b)
+    _chk(gamma, torch.float32, "gamma")
+    if N % 128 != 0 or gamma.numel() != 128:
+        raise ValueError("N must be a multiple of 128 and gamma hold 128 values")
+    if cos_sin is not None:
+        _chk(cos_sin, torch.float32, "cos_sin")
+        if tuple(cos_sin.shape) != (M, 128):
+            raise ValueError(f"cos_sin must have shape {(M, 128)}")
+    out = torch.empty((M, N), device=a.device, dtype=torch.bfloat16)
+    lib = _lib.load()
+    with torch.cuda.device(a.device):
+        _lib.check(lib.g3c_gemm_norm_rope_fp8(a.data_ptr(), scale_a.data_ptr(), b.data_ptr(), scale_b.data_ptr(),
+                                              out.data_ptr(), M, N, K, lda, ldb, N, gamma.data_ptr(), _lib.ptr(cos_sin),
+                                              eps, _lib.stream_ptr()), "g3c_gemm_norm_rope_fp8")
+    return out
+
+
 def attention(q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, heads: int, scale: Optional[float] = None,
               vt_chunk_len: int = 0) -> torch.Tensor:
     """q [Lq, heads*128], k [Lk, heads*128], vt [chunks, heads*128, chunk_len] or [heads*128, Lk] (V transposed).
@@ -136,6 +224,21 @@ def ln_modulate(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, pos: 
         _lib.check(lib.g3c_ln_modulate(_lib.ptr(x), _lib.ptr(pos), _lib.ptr(shift), _lib.ptr(scale), _lib.ptr(y), L, D,
                                        eps, _lib.stream_ptr()), "g3c_ln_modulate")
     return y
+
+
+def ln_modulate_fp8(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, pos: Optional[torch.Tensor] = None,
+                    eps: float = 1e-6) -> tuple[torch.Tensor, torch.Tensor]:
+    """`ln_modulate` with the fp32 result quantised per row as by quantize_rows_fp8 (never rounded to bf16):
+    returns (codes [L, D] torch.float8_e4m3fn, scales [L] float32)."""
+    _chk(x, torch.float32, "x")
+    L, D = x.shape
+    codes = torch.empty((L, D), device=x.device, dtype=torch.float8_e4m3fn)
+    scales = torch.empty(L, device=x.device, dtype=torch.float32)
+    lib = _lib.load()
+    with torch.cuda.device(x.device):
+        _lib.check(lib.g3c_ln_modulate_fp8(_lib.ptr(x), _lib.ptr(pos), _lib.ptr(shift), _lib.ptr(scale), codes.data_ptr(),
+                                           scales.data_ptr(), L, D, eps, _lib.stream_ptr()), "g3c_ln_modulate_fp8")
+    return codes, scales
 
 
 def rmsnorm_rope_(qk: torch.Tensor, heads: int, gamma: torch.Tensor, cos_sin: Optional[torch.Tensor] = None,

@@ -6,7 +6,7 @@
  * reproduces.  Conventions: every pointer is a DEVICE pointer owned by the caller unless noted;
  * `stream` is a cudaStream_t passed as void*; functions enqueue on that stream and return
  * immediately; return 0 on success, <0 on error (G3C_E*), message via g3c_last_error() (thread
- * local).  No hidden allocations after a *_create / *_set_shape / *_set_deterministic call.  Handles are not thread
+ * local).  No hidden allocations after a *_create / *_set_shape / *_set_deterministic / g3c_dit_set_linear_fp8 call.  Handles are not thread
  * safe; distinct handles are independent.  There is no CPU fallback anywhere in this library.
  */
 #ifndef GEN3C_B200_H_
@@ -141,6 +141,24 @@ int g3c_gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, in
 int g3c_gemm_norm_rope_bf16(const void* A, const void* B, void* D, int M, int N, int K, int lda, int ldb, int ldd,
                             const float* gamma, const float* cos_sin, float eps, void* stream);
 
+/* FP8 (e4m3) Linear path.  Row quantisation of bf16 x [R, C] (leading dimension ld): amax_r = max_c |x[r,c]|,
+ * codes[r,c] = e4m3_rn_satfinite(x[r,c] * (448 / amax_r)) (fp32 multiply), scales[r] = amax_r / 448; a zero row gets
+ * codes 0 and scale 1.  C must be a multiple of 16, ld of 8, ldq (>= C) of 16; x, codes, scales 16-byte aligned. */
+int g3c_quantize_rows_fp8(const void* x_bf16, int ld, int R, int C, void* codes, int ldq, float* scales, void* stream);
+
+/* D[M,N] = (A8[M,K] . B8[N,K]^T) * scale_A[m] * scale_B[n], then `epilogue` as in g3c_gemm_bf16: e4m3 codes (K
+ * contiguous) from g3c_quantize_rows_fp8, on the fp8 wgmma; each 128-code k-block's partial sum is added into fp32
+ * accumulators (the instruction's own sum is not full fp32), and tiles are at most 128 columns wide (block_n 256 runs 128).  The scales multiply the accumulators
+ * before any epilogue arithmetic.  K, lda and ldb must be multiples of 16; scale_A [M] and scale_B [N] non-NULL and
+ * 16-byte aligned. */
+int g3c_gemm_fp8(const void* A8, const float* scale_A, const void* B8, const float* scale_B, void* D, int M, int N,
+                 int K, int lda, int ldb, int ldd, int epilogue, const float* gate, int block_n, void* stream);
+
+/* g3c_gemm_norm_rope_bf16 on e4m3 operands: the RMSNorm sees the dequantised accumulators. */
+int g3c_gemm_norm_rope_fp8(const void* A8, const float* scale_A, const void* B8, const float* scale_B, void* D, int M,
+                           int N, int K, int lda, int ldb, int ldd, const float* gamma, const float* cos_sin, float eps,
+                           void* stream);
+
 /* O = softmax(Q K^T * scale) V, head_dim 128, no mask — the attention operator behind
  * Attention.cal_attn (reference: module/attention.py:282-297, TE DotProductAttention :228-238;
  * also usable as an `attn_op`, :136-139).
@@ -174,6 +192,11 @@ int g3c_attn_set_trace(unsigned long long* device_buffer);
  * reference: module/blocks.py:339-341, :547-548 */
 int g3c_ln_modulate(float* x, const void* pos_bf16, const float* shift, const float* scale,
                     void* y_bf16, int L, int D, float eps, void* stream);
+
+/* g3c_ln_modulate with the modulated fp32 rows quantised as in g3c_quantize_rows_fp8: y_codes e4m3 [L,D], y_scales
+ * [L] f32 (both 16-byte aligned, D a multiple of 16).  x is updated as by g3c_ln_modulate. */
+int g3c_ln_modulate_fp8(float* x, const void* pos_bf16, const float* shift, const float* scale, void* y_codes,
+                        float* y_scales, int L, int D, float eps, void* stream);
 
 /* in-place per-head RMSNorm (eps, gamma[128]) and optional rotate-half RoPE (cos_sin [L,128] =
  * cos(angles[0:64]) | sin(angles[0:64])) on bf16 [L, heads*128]
@@ -234,6 +257,15 @@ int g3c_dit_disable_cp(g3c_dit_t* h);
 int g3c_dit_enable_cfg_parallel(g3c_dit_t* h, int role);
 int g3c_dit_cfg_export(g3c_dit_t* h, void* out_handle64);
 int g3c_dit_cfg_import(g3c_dit_t* h, const void* partner_handle64);
+
+/* FP8 Linear mode (off by default).  on != 0: the eight large Linears of every block (self-attention to_q, to_k,
+ * to_v, to_out; cross-attention to_q, to_out; MLP layer1, layer2) run on e4m3 operands with per-row scales: the
+ * weights per output channel, the activations per token (g3c_quantize_rows_fp8 arithmetic).  Allocates the e4m3
+ * weight copies now (about 235 MB per block of the 7B net, 6.6 GB for its 28 blocks); the next forward quantises them
+ * from the registered bf16 weights, and again after every g3c_dit_load.  Frees the shape's workspace: call
+ * g3c_dit_set_shape again (it then also allocates the fp8 activation buffers).  on = 0 frees the copies and returns to the bf16 forward.  Composes with context and CFG
+ * parallelism (K and V^T stay bf16). */
+int g3c_dit_set_linear_fp8(g3c_dit_t* h, int on);
 
 /* Fix the token grid: T_local latent frames on this rank (of T_local*cp_size), latent H x W,
  * context length, fps.  Allocates the workspace and precomputes the abs-pos / RoPE tables. */
