@@ -368,6 +368,9 @@ static int gemm_any(const void* A, const void* B, const float* scale_a, const fl
                     const NormRope* norm_rope) {
   const bool fp8 = scale_a != nullptr;
   G3C_REQUIRE(A && B && D, "gemm: null operand");
+  // only the C ABI's four epilogues are accepted here: EPI_NORM_ROPE_BF16 is selected by `norm_rope` alone (passed as
+  // an epilogue code it would launch the fused norm without a gain vector)
+  G3C_REQUIRE(epilogue >= G3C_EPI_BF16 && epilogue <= G3C_EPI_F32, "gemm: unknown epilogue %d", epilogue);
   if (norm_rope) {
     G3C_REQUIRE(epilogue == G3C_EPI_BF16 && N % 128 == 0 && norm_rope->gamma,
                 "gemm: the RMSNorm/RoPE epilogue needs the bf16 epilogue, N %% 128 == 0 and a gain vector");

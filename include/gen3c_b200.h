@@ -130,7 +130,8 @@ int g3c_render_cache_occlusion(const float* points, const unsigned char* boundar
 
 /* D[M,N] = A[M,K] . B[N,K]^T, bf16 operands (K contiguous), fp32 accumulation on wgmma (Hopper tensor cores).
  * Replaces every nn.Linear of the net (reference: module/attention.py:263-266,289,91-102;
- * module/blocks.py:153-163,228-241).  block_n: 0 = auto, or 64/128/256. */
+ * module/blocks.py:153-163,228-241).  block_n: 0 = auto, or 64/128/256.  epilogue: one of the four G3C_EPI_* above
+ * (any other value is G3C_EINVAL; the fused RMSNorm/RoPE epilogue has its own entry point below). */
 int g3c_gemm_bf16(const void* A, const void* B, void* D, int M, int N, int K, int lda, int ldb,
                   int ldd, int epilogue, const float* gate, int block_n, void* stream);
 
