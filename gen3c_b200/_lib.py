@@ -114,6 +114,8 @@ SIGNATURES = {
     "g3c_dit_profile_wait_ms": (_I, [_P, C.POINTER(_F)]),
     "g3c_dit_workspace_bytes": (C.c_int64, [_P]),
     "g3c_dit_last_launch_count": (_I, [_P]),
+    "g3c_dit_read_tables": (_I, [_P, _I, _P, _P, _P]),
+    "g3c_dit_read_modulation": (_I, [_P, _F, _P, _P, _P]),
 }
 
 _lib = None

@@ -361,8 +361,9 @@ unsigned long long peer_timeout_ns() {
   return v;
 }
 
-static int build_tables(g3c_dit* h, cudaStream_t st) {
-  if (h->tables_ready) return G3C_OK;
+// RoPE cos|sin table [L,128] f32 and abs-pos table [L,D] bf16 of the current shape, for a rank whose first latent frame
+// is t0 (the forward's tables: t0 = cp_rank * T)
+static int write_tables(g3c_dit* h, int t0, float* rope, __nv_bfloat16* pos, cudaStream_t st) {
   const g3c_dit_config& c = h->cfg;
   // RoPE frequencies — reference: position_embedding.py:106-160 (head_dim 128 -> 44 | 42 | 42)
   const int dim = 128, dim_h = dim / 6 * 2, dim_w = dim_h, dim_t = dim - 2 * dim_h;
@@ -376,12 +377,40 @@ static int build_tables(g3c_dit* h, cudaStream_t st) {
   for (int j = 0; j < nw; ++j) fr[nt + nh + j] = 1.0f / powf(th_w, (float)(2 * j) / (float)dim_w);
   G3C_CUDA(cudaMemcpyAsync(h->freqs, fr.data(), 64 * sizeof(float), cudaMemcpyHostToDevice, st));
   G3C_CUDA(cudaStreamSynchronize(st));  // fr is a stack-lifetime host buffer
-  const int t0 = h->cp_rank * h->T;
   // seq[:T] / fps * base_fps  (position_embedding.py:163)
   const float t_scale = (1.0f / h->fps) * (float)c.base_fps;
-  TRY(rope_table(h->freqs, nt, nh, nw, t0, t_scale, h->T, h->Hp, h->Wp, h->rope, st));
-  TRY(abs_pos(h->pos_t, h->pos_h, h->pos_w, t0, h->T, h->Hp, h->Wp, c.model_channels, h->pos, st));
+  TRY(rope_table(h->freqs, nt, nh, nw, t0, t_scale, h->T, h->Hp, h->Wp, rope, st));
+  TRY(abs_pos(h->pos_t, h->pos_h, h->pos_w, t0, h->T, h->Hp, h->Wp, c.model_channels, pos, st));
+  return G3C_OK;
+}
+
+static int build_tables(g3c_dit* h, cudaStream_t st) {
+  if (h->tables_ready) return G3C_OK;
+  TRY(write_tables(h, h->cp_rank * h->T, h->rope, h->pos, st));
   h->tables_ready = true;
+  return G3C_OK;
+}
+
+// timestep embedding + all adaLN-LoRA modulation vectors (blocks.py:38-80, :442-445; general_dit.py:405) into h->mods /
+// h->modf.  They depend on t only: the cond and uncond forwards of one denoise step share t (model_v2w.py:140-142), so
+// they are computed once per timestep.  n counts the launches.
+static int modulation(g3c_dit* h, float timestep, int& n, cudaStream_t st) {
+  if (h->mods_valid && h->mods_timestep == timestep) return G3C_OK;
+  const g3c_dit_config& c = h->cfg;
+  const int D = c.model_channels, R = c.adaln_lora_dim;
+  K(CAT_VECTOR, timestep_embed(timestep, D, h->affine_gamma, 1e-6f, h->vec_s, h->vec_emb, st));
+  K(CAT_VECTOR, gemv(h->w_t1, h->vec_s, nullptr, h->vec_h1, D, D, 0, 0, st));
+  K(CAT_VECTOR, gemv(h->w_t2, h->vec_h1, nullptr, h->vec_lora, 3 * D, D, 1, 0, st));
+  for (int i = 0; i < c.num_blocks; ++i)
+    for (int j = 0; j < 3; ++j) {
+      const SubBlock& s = h->blk[i][j];
+      K(CAT_VECTOR, gemv(s.ada1, h->vec_emb, nullptr, h->vec_a, R, D, 1, 0, st));
+      K(CAT_VECTOR, gemv(s.ada2, h->vec_a, h->vec_lora, h->mods + (size_t)(i * 3 + j) * 3 * D, 3 * D, R, 0, 0, st));
+    }
+  K(CAT_VECTOR, gemv(h->f_ada1, h->vec_emb, nullptr, h->vec_a, R, D, 1, 0, st));
+  K(CAT_VECTOR, gemv(h->f_ada2, h->vec_a, h->vec_lora, h->modf, 2 * D, R, 0, 0, st));
+  h->mods_valid = true;
+  h->mods_timestep = timestep;
   return G3C_OK;
 }
 
@@ -394,7 +423,7 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
   TRY(resolve(h, st));
   TRY(build_tables(h, st));
   const g3c_dit_config& c = h->cfg;
-  const int D = c.model_channels, R = c.adaln_lora_dim, F = c.ffn_dim, L = h->L, heads = c.num_heads;
+  const int D = c.model_channels, F = c.ffn_dim, L = h->L, heads = c.num_heads;
   const int Lk_all = L * h->cp_size;
   const float attn_scale = 0.6931471805599453f;  // ln 2: 1/sqrt(128) * log2(e) is folded into the query RMSNorm gain
   // to_q / to_k: Linear + per-head RMSNorm (+ RoPE), fused into the GEMM epilogue: the norm and the rotation act on the
@@ -438,24 +467,8 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
   K(CAT_ELTWISE, patchify(src, h->T, h->Hp, h->Wp, h->Kpad, h->tok, st));
   K(CAT_GEMM, gemm_bf16(h->tok, h->w_patch_pad, h->x, L, D, h->Kpad, h->Kpad, h->Kpad, D, G3C_EPI_F32, nullptr, 0, st));
 
-  // ---- timestep embedding + all adaLN-LoRA modulation vectors (blocks.py:38-80, :442-445;
-  //      general_dit.py:405).  They depend on t only.
-  //      cond and uncond forward of one denoise step share t (model_v2w.py:140-142): computed once per timestep.
-  if (!(h->mods_valid && h->mods_timestep == timestep)) {
-    K(CAT_VECTOR, timestep_embed(timestep, D, h->affine_gamma, 1e-6f, h->vec_s, h->vec_emb, st));
-    K(CAT_VECTOR, gemv(h->w_t1, h->vec_s, nullptr, h->vec_h1, D, D, 0, 0, st));
-    K(CAT_VECTOR, gemv(h->w_t2, h->vec_h1, nullptr, h->vec_lora, 3 * D, D, 1, 0, st));
-    for (int i = 0; i < c.num_blocks; ++i)
-      for (int j = 0; j < 3; ++j) {
-        const SubBlock& s = h->blk[i][j];
-        K(CAT_VECTOR, gemv(s.ada1, h->vec_emb, nullptr, h->vec_a, R, D, 1, 0, st));
-        K(CAT_VECTOR, gemv(s.ada2, h->vec_a, h->vec_lora, h->mods + (size_t)(i * 3 + j) * 3 * D, 3 * D, R, 0, 0, st));
-      }
-    K(CAT_VECTOR, gemv(h->f_ada1, h->vec_emb, nullptr, h->vec_a, R, D, 1, 0, st));
-    K(CAT_VECTOR, gemv(h->f_ada2, h->vec_a, h->vec_lora, h->modf, 2 * D, R, 0, 0, st));
-    h->mods_valid = true;
-    h->mods_timestep = timestep;
-  }
+  // ---- timestep embedding + adaLN-LoRA modulation vectors (cached per timestep)
+  TRY(modulation(h, timestep, n, st));
 
   __nv_bfloat16* k_loc = h->k_all + (size_t)h->cp_rank * L * D;
   __nv_bfloat16* vt_loc = h->vt_all + (size_t)h->cp_rank * L * D;
@@ -1006,5 +1019,30 @@ int g3c_dit_profile_read(g3c_dit_t* h, float* ms_by_category, int* launches_by_c
 
 int64_t g3c_dit_workspace_bytes(const g3c_dit_t* h) { return h ? (int64_t)(h->ws_bytes + h->w8_bytes) : 0; }
 int g3c_dit_last_launch_count(const g3c_dit_t* h) { return h ? h->launches : 0; }
+
+// ---- C ABI test hooks for the engine's derived tables and vectors --------------------------------
+int g3c_dit_read_tables(g3c_dit_t* h, int t0, float* rope, void* pos, void* stream) {
+  G3C_REQUIRE(h && rope && pos, "dit_read_tables: null argument");
+  G3C_REQUIRE(h->L > 0, "dit_read_tables: g3c_dit_set_shape was not called");
+  G3C_REQUIRE(t0 >= 0 && t0 + h->T <= h->cfg.max_frames, "dit_read_tables: frames [%d, %d) exceed max_frames=%d", t0,
+              t0 + h->T, h->cfg.max_frames);
+  cudaStream_t st = (cudaStream_t)stream;
+  TRY(resolve(h, st));
+  return write_tables(h, t0, rope, (__nv_bfloat16*)pos, st);
+}
+
+int g3c_dit_read_modulation(g3c_dit_t* h, float timestep, float* mods, float* modf, void* stream) {
+  G3C_REQUIRE(h && mods && modf, "dit_read_modulation: null argument");
+  G3C_REQUIRE(h->L > 0, "dit_read_modulation: g3c_dit_set_shape was not called");
+  cudaStream_t st = (cudaStream_t)stream;
+  TRY(resolve(h, st));
+  int n = 0;
+  TRY(modulation(h, timestep, n, st));
+  const size_t D = h->cfg.model_channels;
+  G3C_CUDA(cudaMemcpyAsync(mods, h->mods, (size_t)h->cfg.num_blocks * 3 * 3 * D * sizeof(float),
+                           cudaMemcpyDeviceToDevice, st));
+  G3C_CUDA(cudaMemcpyAsync(modf, h->modf, 2 * D * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return G3C_OK;
+}
 
 }  // extern "C"

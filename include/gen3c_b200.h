@@ -320,6 +320,17 @@ int64_t g3c_dit_workspace_bytes(const g3c_dit_t* h);
 /* number of kernels the last g3c_dit_forward enqueued (for bench.py's gpu_launches) */
 int g3c_dit_last_launch_count(const g3c_dit_t* h);
 
+/* ---- test hooks: read back what the forward derives from the weights, the shape and the timestep ---- */
+/* The position tables of the current shape (g3c_dit_set_shape), built as a rank whose first latent frame is t0 builds
+ * them: rope f32 [L,128] = cos | sin of the angles (t | h | w columns 22 | 21 | 21, token (t*Hp + h)*Wp + w), pos bf16
+ * [L,D] the per-block abs-pos embedding.  The forward uses t0 = cp_rank * T_local.  t0 + T_local > max_frames is
+ * G3C_EINVAL.  Leaves the forward's own tables untouched. */
+int g3c_dit_read_tables(g3c_dit_t* h, int t0, float* rope, void* pos, void* stream);
+/* The adaLN modulation vectors a forward at `timestep` uses: mods f32 [num_blocks*3][3D] (shift | scale | gate of
+ * block i, sub-block j at row i*3 + j), modf f32 [2D] (final layer shift | scale).  Goes through the forward's
+ * per-timestep cache (a forward right after at the same timestep reuses the vectors). */
+int g3c_dit_read_modulation(g3c_dit_t* h, float timestep, float* mods, float* modf, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
