@@ -17,8 +17,9 @@
 //   warpgroups 1-2  consumers, 64 query rows each, software-pipelined with one S tile of lookahead:
 //                     prologue  S_0 = Q K_0^T, softmax, pack P_0
 //                     step j    [turn] issue S_j = Q K_j^T and O += P_{j-1} V_{j-1} [pass turn]; wait<1> (S_j done,
-//                               release K_j); row max and 2^(s - m) of S_j in place; wait<0> (P.V done, release
-//                               V_{j-1}); rescale O and l; pack P_j (bf16 A fragments of the next P.V, from registers)
+//                               release K_j); row max and 2^(s - m) of S_j in place (m moves lazily, softmax_tile);
+//                               wait<0> (P.V done, release V_{j-1}); rescale O if m moved; pack P_j (bf16 A fragments
+//                               of the next P.V, from registers)
 //                     epilogue  [turn] O += P_{n-1} V_{n-1} [pass turn]; wait<0>; normalise and store
 //                   so the softmax of step j runs under this warpgroup's own P.V(j-1).  Between the two warpgroups a turn
 //                   token (two mbarriers) alternates the MMA issue, so one warpgroup's softmax sits under the other's
@@ -42,6 +43,11 @@ constexpr int ATT_STAGES = 2;
 constexpr int ATT_SMEM = ATT_TILE_BYTES + ATT_STAGES * 2 * ATT_TILE_BYTES + 256 + 1024;
 static_assert(ATT_SMEM <= 227 * 1024, "attention: Q + K/V rings exceed the 227 KB of shared memory per block");
 static_assert(1 + 4 * ATT_STAGES + 3 <= 256 / 8, "attention: barriers exceed their 256-byte area");
+// The consumers' steady-state loop is unrolled by the ring depth, so every stage index and parity in it is a constant.
+static_assert(ATT_STAGES == 2, "attention: the consumer loop is unrolled for a ring depth of 2");
+// Lazy rescale (softmax_tile): the reference row max moves only when a row's tile max exceeds it by more than this many
+// powers of two, so P <= 2^8 between moves.
+constexpr float ATT_RESCALE_LOG2 = 8.0f;
 
 struct AttnParams {
   int Lq, Lk, heads;
@@ -75,9 +81,14 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return y;
 }
 
-// Online softmax of one S tile (this thread's two rows): exact row max of the tile, new running max m, correction
-// alpha = 2^(m_old - m_new), and S <- 2^(S sl2 - m_new) in place with the row sums l <- l alpha + sum.
-__device__ __forceinline__ void softmax_tile(float (&s)[64], float (&m_run)[2], float (&l_run)[2], float (&alpha)[2],
+// Online softmax of one S tile (this thread's two rows), with a lazy reference.  The row max of the tile is exact; the
+// reference m the exponentials are taken against only moves when some row of the warp's 16 exceeds its m by more than
+// ATT_RESCALE_LOG2 (log2 units).  Then m <- max(m, row max), alpha = 2^(m_old - m_new), l <- l alpha, and the function
+// returns true: the caller rescales O by alpha.  Otherwise (most tiles once the first few have set m) it returns false,
+// and P = 2^(S sl2 - m) <= 2^ATT_RESCALE_LOG2 against the stale m, which bf16 P and the fp32 row sums hold with room to
+// spare.  The first tile always moves m (m = -inf).  The decision is a warp vote, so the branch on it stays uniform.
+// S <- P in place, l <- l + row sums of P.
+__device__ __forceinline__ bool softmax_tile(float (&s)[64], float (&m_ref)[2], float (&l_run)[2], float (&alpha)[2],
                                              float sl2) {
   float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
@@ -85,56 +96,65 @@ __device__ __forceinline__ void softmax_tile(float (&s)[64], float (&m_run)[2], 
     mx[0] = fmaxf(mx[0], fmaxf(s[4 * i], s[4 * i + 1]));
     mx[1] = fmaxf(mx[1], fmaxf(s[4 * i + 2], s[4 * i + 3]));
   }
-  float nm[2];
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
     mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
-    nm[h] = fmaxf(m_run[h], mx[h] * sl2);
-    alpha[h] = ex2_approx(m_run[h] - nm[h]);  // 0 on the first tile (m_run = -inf)
-    m_run[h] = nm[h];
-    l_run[h] *= alpha[h];
+    mx[h] *= sl2;
   }
+  const bool keep = __all_sync(0xffffffffu, mx[0] - m_ref[0] <= ATT_RESCALE_LOG2 && mx[1] - m_ref[1] <= ATT_RESCALE_LOG2);
+  if (!keep) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const float nm = fmaxf(m_ref[h], mx[h]);
+      alpha[h] = ex2_approx(m_ref[h] - nm);  // 0 on the first tile (m = -inf)
+      m_ref[h] = nm;
+      l_run[h] *= alpha[h];
+    }
+  }
+  const float nm0 = -m_ref[0], nm1 = -m_ref[1];
 #pragma unroll
   for (int i = 0; i < 16; ++i) {
-    s[4 * i] = ex2_approx(fmaf(s[4 * i], sl2, -nm[0]));
-    s[4 * i + 1] = ex2_approx(fmaf(s[4 * i + 1], sl2, -nm[0]));
-    s[4 * i + 2] = ex2_approx(fmaf(s[4 * i + 2], sl2, -nm[1]));
-    s[4 * i + 3] = ex2_approx(fmaf(s[4 * i + 3], sl2, -nm[1]));
+    s[4 * i] = ex2_approx(fmaf(s[4 * i], sl2, nm0));
+    s[4 * i + 1] = ex2_approx(fmaf(s[4 * i + 1], sl2, nm0));
+    s[4 * i + 2] = ex2_approx(fmaf(s[4 * i + 2], sl2, nm1));
+    s[4 * i + 3] = ex2_approx(fmaf(s[4 * i + 3], sl2, nm1));
     l_run[0] += s[4 * i] + s[4 * i + 1];
     l_run[1] += s[4 * i + 2] + s[4 * i + 3];
   }
+  return !keep;
+}
+
+// The wgmma shared-memory descriptors of this kernel, split in two 32-bit words: the low word carries the start address
+// (and the LBO of the MN-major V tile), the high word is the same for all of them (SBO 1024 B, SWIZZLE_128B; see
+// make_sdesc_sw128).  A k-step offset is added to the low word alone: the 14-bit address field of a shared-memory
+// address plus an offset inside its tile never carries out.  The loop-invariant low words are computed once per CTA.
+constexpr uint32_t ATT_SDESC_HI = (1024u >> 4) | (1u << 30);
+__device__ __forceinline__ uint64_t sdesc_at(uint32_t lo, uint32_t bytes) {
+  return (static_cast<uint64_t>(ATT_SDESC_HI) << 32) | (lo + (bytes >> 4));
 }
 
 // S = Q K^T of one KV tile: 8 k-steps over the head dimension, A (Q rows of this warpgroup) and B (K tile) in shared memory
-__device__ __forceinline__ void issue_s(float (&s)[64], uint64_t dq, const uint8_t* k_tile) {
-  const uint64_t dk = make_sdesc_sw128(smem_u32(k_tile));
+__device__ __forceinline__ void issue_s(float (&s)[64], uint32_t dq, uint32_t dk) {
 #pragma unroll
   for (int kk = 0; kk < 8; ++kk) {  // head dimensions 16 kk .. 16 kk + 15
     const uint32_t off = (kk >> 2) * ATT_HALF_BYTES + (kk & 3) * 32;
-    wgmma_ss_n128(s, sdesc_advance(dq, off), sdesc_advance(dk, off), kk > 0 ? 1u : 0u);
+    wgmma_ss_n128(s, sdesc_at(dq, off), sdesc_at(dk, off), kk > 0 ? 1u : 0u);
   }
 }
 
 // O += P V of one KV tile: P from registers (bf16 A fragments), V in shared memory.  V^T tile (keys contiguous): K-major
 // B.  Token-major V tile (kVTokenMajor; head dims contiguous, loaded like K): MN-major B whose two 64-dim halves are
-// ATT_HALF_BYTES apart (LBO), and k-step kk starts 16 keys of 128-byte rows into each half.
+// ATT_HALF_BYTES apart (LBO, in `dv`), and k-step kk starts 16 keys of 128-byte rows into each half.
 template <bool kVTokenMajor>
-__device__ __forceinline__ void issue_pv(float (&o)[64], const uint32_t (&pa)[32], const uint8_t* v_tile) {
-  if constexpr (kVTokenMajor) {
-    const uint64_t dv = make_sdesc_sw128_mn(smem_u32(v_tile), ATT_HALF_BYTES);
+__device__ __forceinline__ void issue_pv(float (&o)[64], const uint32_t (&pa)[32], uint32_t dv) {
 #pragma unroll
-    for (int kk = 0; kk < 8; ++kk) {
-      const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
-      wgmma_rs_n128_tb(o, a, sdesc_advance(dv, kk * 16 * 128));
-    }
-  } else {
-    const uint64_t dv = make_sdesc_sw128(smem_u32(v_tile));
-#pragma unroll
-    for (int kk = 0; kk < 8; ++kk) {  // keys 16 kk .. 16 kk + 15 = accumulator columns of S
-      const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
-      wgmma_rs_n128(o, a, sdesc_advance(dv, (kk >> 2) * ATT_HALF_BYTES + (kk & 3) * 32));
-    }
+  for (int kk = 0; kk < 8; ++kk) {  // keys 16 kk .. 16 kk + 15 = accumulator columns of S
+    const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
+    if constexpr (kVTokenMajor)
+      wgmma_rs_n128_tb(o, a, sdesc_at(dv, kk * 16 * 128));
+    else
+      wgmma_rs_n128(o, a, sdesc_at(dv, (kk >> 2) * ATT_HALF_BYTES + (kk & 3) * 32));
   }
 }
 
@@ -261,7 +281,8 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
   } else {
     // ===== consumers: warpgroup c owns query rows [64c, 64c + 64) of the tile =====
     setmaxnreg_inc<240>();
-    const uint32_t c = wg - 1;
+    const uint32_t c = __shfl_sync(0xffffffffu, wg - 1, 0);  // warp-uniform for the compiler: descriptors and barrier
+                                                               // addresses derived from it stay in uniform registers
     const uint32_t warp = tid / 32, lane = tid % 32;
     const unsigned long long tmo = p.peer_timeout_ns;
     // accumulator layout (wgmma m64n128k16, f32), i in [0, 16): acc[4i + {0,1}] = row 16 warp + lane/4, columns 8i + 2 (lane%4) + {0,1};
@@ -271,109 +292,72 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
     for (int i = 0; i < 64; ++i) o[i] = 0.f;
     float s[64];      // S_j, then 2^(S_j - m) in place
     uint32_t pa[32];  // P_{j-1}: the A operand of the P.V in flight during the softmax of step j
-    float m_run[2] = {-INFINITY, -INFINITY};  // running row max (log2 units) of the two rows of this thread
+    float m_ref[2] = {-INFINITY, -INFINITY};  // reference row max (log2 units) of the two rows of this thread
     float l_run[2] = {0.f, 0.f};              // this thread's partial row sums (quad-reduced at the end)
     float alpha[2];
     const float sl2 = p.scale_log2;
-    const uint64_t dq = make_sdesc_sw128(smem_u32(smem_q + c * 64 * 128));
-    uint32_t tph = 0;         // parity of this warpgroup's next turn (turn t waits for phase t of turn[c])
-    uint32_t ks = 0, kp = 0;  // ring stage / parity of K_j
-    uint32_t vs = 0, vp = 0;  // ring stage / parity of V_{j-1}
+    // descriptor low words (sdesc_at): this warpgroup's Q rows, and the K and V tile of each ring stage
+    const uint32_t dq = (uint32_t)make_sdesc_sw128(smem_u32(smem_q + c * 64 * 128));
+    uint32_t dk[ATT_STAGES], dv[ATT_STAGES];
+#pragma unroll
+    for (int st = 0; st < ATT_STAGES; ++st) {
+      dk[st] = (uint32_t)make_sdesc_sw128(smem_u32(smem_k + st * ATT_TILE_BYTES));
+      dv[st] = (uint32_t)(kVTokenMajor ? make_sdesc_sw128_mn(smem_u32(smem_v + st * ATT_TILE_BYTES), ATT_HALF_BYTES)
+                                       : make_sdesc_sw128(smem_u32(smem_v + st * ATT_TILE_BYTES)));
+    }
+    // Ring positions as functions of the KV tile: K_j sits in stage j % 2 at parity (j / 2) % 2, V_{j-1} in stage
+    // (j - 1) % 2 at parity ((j - 1) / 2) % 2, and this warpgroup's turn t waits for parity t % 2 of turn[c] (turn j is
+    // taken at step j).
     int j = 0;
     // ---- prologue: S_0, softmax, P_0 ----
     mbar_wait_ns_or_exit(q_full, 0, tmo);
-    mbar_wait_ns_or_exit(&k_full[ks], kp, tmo);
-    mbar_wait_ns_or_exit(&turn[c], tph, tmo);
-    tph ^= 1;
+    mbar_wait_ns_or_exit(&k_full[0], 0, tmo);
+    mbar_wait_ns_or_exit(&turn[c], 0, tmo);
     ATT_TR(1 + c, 0);
     wgmma_fence();
-    issue_s(s, dq, smem_k + ks * ATT_TILE_BYTES);
+    issue_s(s, dq, dk[0]);
     wgmma_commit();
     if (lane == 0) mbar_arrive(&turn[c ^ 1]);
     ATT_TR(1 + c, 1);
     wgmma_wait<0>();
     fence_regs(s);
-    if (tid == 0) mbar_arrive(&k_empty[ks]);
+    if (tid == 0) mbar_arrive(&k_empty[0]);
     ATT_TR(1 + c, 2);
     if constexpr (kVTokenMajor) {
       if (n_kv == 1) mask_key_tail(s, p.Lk, lane);
     }
-    softmax_tile(s, m_run, l_run, alpha, sl2);
+    softmax_tile(s, m_ref, l_run, alpha, sl2);  // sets m: O and l are still 0
     pack_p(pa, s);
     ATT_TR(1 + c, 3);
-    if (++ks == ATT_STAGES) {
-      ks = 0;
-      kp ^= 1;
-    }
-    // ---- steady state: S_j is computed while P.V(j-1) runs; the softmax of S_j runs under P.V(j-1) ----
-    for (j = 1; j < (kVTokenMajor ? n_kv - 1 : n_kv); ++j) {
-      mbar_wait_ns_or_exit(&k_full[ks], kp, tmo);
-      mbar_wait_ns_or_exit(&v_full[vs], vp, tmo);
-      mbar_wait_ns_or_exit(&turn[c], tph, tmo);
-      tph ^= 1;
+    // ---- step j: S_j is computed while P.V(j-1) runs; the softmax of S_j runs under P.V(j-1).  K_j in stage kst at
+    // parity kpar, V_{j-1} in stage vst at parity vpar, turn parity j % 2; keys of the tile from `valid` on are masked
+    // (valid < ATT_TILE only in the last tile of a ragged token-major Lk) ----
+    auto step = [&](int kst, int vst, uint32_t kpar, uint32_t vpar, int valid) {
+      mbar_wait_ns_or_exit(&k_full[kst], kpar, tmo);
+      mbar_wait_ns_or_exit(&v_full[vst], vpar, tmo);
+      mbar_wait_ns_or_exit(&turn[c], (uint32_t)j & 1u, tmo);
       ATT_TR(1 + c, 0);
       wgmma_fence();
-      issue_s(s, dq, smem_k + ks * ATT_TILE_BYTES);
+      issue_s(s, dq, kst ? dk[1] : dk[0]);
       wgmma_commit();
-      issue_pv<kVTokenMajor>(o, pa, smem_v + vs * ATT_TILE_BYTES);
+      issue_pv<kVTokenMajor>(o, pa, vst ? dv[1] : dv[0]);
       wgmma_commit();
       if (lane == 0) mbar_arrive(&turn[c ^ 1]);
       ATT_TR(1 + c, 1);
       wgmma_wait<1>();  // S_j complete; P.V(j-1) may still run
       fence_regs(s);
-      if (tid == 0) mbar_arrive(&k_empty[ks]);
+      if (tid == 0) mbar_arrive(&k_empty[kst]);
       ATT_TR(1 + c, 2);
-      softmax_tile(s, m_run, l_run, alpha, sl2);  // P_{j-1} (pa) and O are still read / written by the P.V in flight
+      if (valid < ATT_TILE) mask_key_tail(s, valid, lane);
+      // P_{j-1} (pa) and O are still read / written by the P.V in flight
+      const bool rescale = softmax_tile(s, m_ref, l_run, alpha, sl2);
       ATT_TR(1 + c, 3);
       wgmma_wait<0>();
       fence_regs(o);
       fence_regs(pa);  // pa stays allocated (not reused for the exponentials above) until the P.V has read it
-      if (tid == 0) mbar_arrive(&v_empty[vs]);
+      if (tid == 0) mbar_arrive(&v_empty[vst]);
       ATT_TR(1 + c, 4);
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        o[4 * i] *= alpha[0];
-        o[4 * i + 1] *= alpha[0];
-        o[4 * i + 2] *= alpha[1];
-        o[4 * i + 3] *= alpha[1];
-      }
-      pack_p(pa, s);
-      if (++ks == ATT_STAGES) {
-        ks = 0;
-        kp ^= 1;
-      }
-      if (++vs == ATT_STAGES) {
-        vs = 0;
-        vp ^= 1;
-      }
-    }
-    if constexpr (kVTokenMajor) {
-      // ---- the last KV tile, peeled off the loop: the same step with the keys past Lk masked before the row max ----
-      if (n_kv > 1) {
-        mbar_wait_ns_or_exit(&k_full[ks], kp, tmo);
-        mbar_wait_ns_or_exit(&v_full[vs], vp, tmo);
-        mbar_wait_ns_or_exit(&turn[c], tph, tmo);
-        tph ^= 1;
-        ATT_TR(1 + c, 0);
-        wgmma_fence();
-        issue_s(s, dq, smem_k + ks * ATT_TILE_BYTES);
-        wgmma_commit();
-        issue_pv<kVTokenMajor>(o, pa, smem_v + vs * ATT_TILE_BYTES);
-        wgmma_commit();
-        if (lane == 0) mbar_arrive(&turn[c ^ 1]);
-        ATT_TR(1 + c, 1);
-        wgmma_wait<1>();  // S_j complete; P.V(j-1) may still run
-        fence_regs(s);
-        if (tid == 0) mbar_arrive(&k_empty[ks]);
-        ATT_TR(1 + c, 2);
-        mask_key_tail(s, p.Lk - j * ATT_TILE, lane);
-        softmax_tile(s, m_run, l_run, alpha, sl2);
-        ATT_TR(1 + c, 3);
-        wgmma_wait<0>();
-        fence_regs(o);
-        fence_regs(pa);  // pa stays allocated (not reused for the exponentials above) until the P.V has read it
-        if (tid == 0) mbar_arrive(&v_empty[vs]);
-        ATT_TR(1 + c, 4);
+      if (rescale) {  // warp-uniform
 #pragma unroll
         for (int i = 0; i < 16; ++i) {
           o[4 * i] *= alpha[0];
@@ -381,27 +365,41 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
           o[4 * i + 2] *= alpha[1];
           o[4 * i + 3] *= alpha[1];
         }
-        pack_p(pa, s);
-        if (++vs == ATT_STAGES) {
-          vs = 0;
-          vp ^= 1;
-        }
+      }
+      pack_p(pa, s);
+    };
+    // ---- steady state, two steps per iteration: j = 2u + 1 (K stage 1, V stage 0) and j = 2u + 2 (K stage 0, V
+    // stage 1); `ph` = u % 2 ----
+    const int j_end = kVTokenMajor ? n_kv - 1 : n_kv;  // the token-major build peels the last tile off (masked)
+    uint32_t ph = 0;
+    for (j = 1; j < j_end; ++j) {
+      step(1, 0, ph, ph, ATT_TILE);
+      if (++j == j_end) break;
+      step(0, 1, ph ^ 1u, ph, ATT_TILE);
+      ph ^= 1u;
+    }
+    if constexpr (kVTokenMajor) {
+      // ---- the last KV tile: the same step with the keys past Lk masked before the row max ----
+      if (n_kv > 1) {
+        j = n_kv - 1;
+        step(j & 1, (j - 1) & 1, ((uint32_t)j >> 1) & 1u, ((uint32_t)(j - 1) >> 1) & 1u, p.Lk - j * ATT_TILE);
       }
       j = n_kv;
     }
     // ---- epilogue: O += P_{n-1} V_{n-1} (the last turn: both warpgroups take n_kv + 1 turns) ----
-    mbar_wait_ns_or_exit(&v_full[vs], vp, tmo);
-    mbar_wait_ns_or_exit(&turn[c], tph, tmo);
+    const int vst = (n_kv - 1) & 1;
+    mbar_wait_ns_or_exit(&v_full[vst], ((uint32_t)(n_kv - 1) >> 1) & 1u, tmo);
+    mbar_wait_ns_or_exit(&turn[c], (uint32_t)n_kv & 1u, tmo);
     ATT_TR(1 + c, 0);
     wgmma_fence();
-    issue_pv<kVTokenMajor>(o, pa, smem_v + vs * ATT_TILE_BYTES);
+    issue_pv<kVTokenMajor>(o, pa, vst ? dv[1] : dv[0]);
     wgmma_commit();
     if (lane == 0) mbar_arrive(&turn[c ^ 1]);
     ATT_TR(1 + c, 1);
     wgmma_wait<0>();
     fence_regs(o);
     fence_regs(pa);
-    if (tid == 0) mbar_arrive(&v_empty[vs]);
+    if (tid == 0) mbar_arrive(&v_empty[vst]);
     ATT_TR(1 + c, 4);
     // ---- normalise and store ----
     float inv[2];
