@@ -68,6 +68,9 @@ __device__ __forceinline__ SplatIdx splat_indices(float flow_x, float flow_y, in
   return s;
 }
 
+// fmaxf(NaN, 0) = 0: a NaN depth contributes log-depth 0, so it never reaches the group max.  Such a source also fails
+// q_z > 0 and splats with weight 0: a NaN point is dropped, like a point behind the camera.  (The reference's
+// torch.clamp / torch.max would propagate it and turn every weight of the chunk into NaN.)  +Inf gives +Inf.
 __device__ __forceinline__ float log_depth(float z) { return log1pf(fmaxf(z, 0.0f)); }
 
 __device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
@@ -76,7 +79,7 @@ __device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float 
                : "memory");
 }
 
-// lz >= 0 or NaN, so the int ordering of the bit pattern equals the float ordering.
+// lz >= 0 (log_depth never returns NaN), so the int ordering of the bit pattern equals the float ordering.
 __device__ __forceinline__ void block_atomic_max(float v, float* dst) {
   __shared__ float red[32];
   v = warp_max(v);
@@ -119,7 +122,7 @@ __global__ void __launch_bounds__(256) k_project_max(const float* __restrict__ p
     float qx, qy, qz;
     project(c, p[3 * i], p[3 * i + 1], p[3 * i + 2], qx, qy, qz);
     float lz = log_depth(qz);
-    m = (lz > m || lz != lz) ? lz : m;  // propagate NaN like torch.max
+    m = (lz > m || lz != lz) ? lz : m;  // lz is never NaN (log_depth drops NaN depths)
   }
   block_atomic_max(m, gmax + item / group);
 }
@@ -154,7 +157,7 @@ __global__ void __launch_bounds__(256)
         float qx, qy, qz;
         project(c, px[j], py[j], pz[j], qx, qy, qz);
         const float lz = log_depth(qz);
-        m = (lz > m || lz != lz) ? lz : m;  // propagate NaN like torch.max
+        m = (lz > m || lz != lz) ? lz : m;  // lz is never NaN (log_depth drops NaN depths)
       }
     m = warp_max(m);
     if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<int*>(&smax[f]), __float_as_int(m));
@@ -260,8 +263,9 @@ __global__ void __launch_bounds__(256)
 // pixel and 4 vector reds.  Here:
 //  * per pixel 2 IEEE divisions (the projected coordinates: their floor / ceil pick the destination, kept exact), one
 //    LG2, one EX2, one RCP: dw = exp(50 lz / lzmax) is inverted once (rcp.approx, 1 ulp) and multiplies the four
-//    bilinear weights; 50 / (lzmax + 1e-7) is a per-item constant; log1p(z) = lg2(1 + z) ln 2 — absolute error
-//    2.4e-7, i.e. 1e-5 relative on a weight, far inside the parity tolerance (the weights are normalised away);
+//    bilinear weights; 50 / (lzmax + 1e-7) is a per-item constant; log1p(z) = lg2(1 + z) ln 2 — its absolute error is
+//    multiplied by 50 / lzmax, so a weight's relative error grows as the depth range shrinks (1.2e-4 derived at depths
+//    of 0.02, DESIGN.md §3.4); tests/test_render_edges_gpu.py holds every pixel to the bound that follows;
 //  * a thread walks 4 neighbouring source pixels of one row and keeps one pending destination per output row in
 //    registers: under a smooth warp the north-east corner of pixel j is the north-west corner of pixel j+1, so a thread
 //    issues ~10 vector reds for 4 pixels instead of 16 (contributions to the same texel are added in registers first).
@@ -346,7 +350,7 @@ __global__ void __launch_bounds__(256)
       const float zc = fmaxf(qz, 0.0f);
       const float lz = __log2f(1.0f + zc) * 0.6931471805599453f;
       const float e = fminf(lz * escale, 80.0f);
-      // m / (exp(e) + 1e-7); NaN depths propagate like the reference's (NaN weights, nan_to_num in the normalise pass)
+      // m / (exp(e) + 1e-7); a NaN depth has m = 0 and zc = 0, so its weights are 0 (dropped, as in log_depth)
       const float rdw = m * rcp_approx(__fadd_rn(ex2_fast(e * 1.4426950408889634f), 1e-7f));
       const long long rt = (long long)s.fy * Wp, rb = (long long)s.cy * Wp;
       pend_add(top, rt + s.fx, dyf * dxf * rdw, v0[j], v1[j], v2[j], qz, a, az);
