@@ -12,9 +12,11 @@
 //   att    bf16 [L, D]        hid  bf16 [L, ffn]
 //   pos    bf16 [L, D]        per-block absolute position embedding (precomputed per shape)
 //   rope   f32  [L, 128]      cos|sin table (precomputed per shape)
-// Context parallelism: tokens are split contiguously along latent T (module/parallel.py:44-53);
-// per self-attention layer K and V^T of every rank are all-gathered in place (one ncclAllGather
-// each, same result as the reference's TE ring: general_dit.py:524-543).
+// Context parallelism: tokens are split contiguously along latent T (module/parallel.py:44-53), and every
+// self-attention layer gathers the K and V^T of all ranks (same result as the reference's TE ring:
+// general_dit.py:524-543).  Default (p2p): each rank projects its K / V^T slice into its slot of a peer-mapped region,
+// the copy engines push the slice to every peer and raise an arrival flag there, and attention reads each remote chunk
+// once its flag is up.  NCCL mode (G3C_CP_MODE=nccl): one in-place ncclAllGather of K and one of V^T per layer.
 #include <dlfcn.h>
 
 #include <array>
@@ -23,6 +25,7 @@
 #include <cstring>
 #include <string>
 #include <unordered_map>
+#include <utility>
 #include <vector>
 
 #include "kernels.h"
@@ -80,20 +83,41 @@ struct WTensor {
   int dtype = 0;
 };
 
-// engine-owned e4m3 copy of one Linear weight [N, K]: codes + per-output-channel scales [N]
-struct W8 {
+// One Linear weight [N, K]: the registered bf16 tensor and, in the fp8 Linear mode, the engine's e4m3 copy of it
+// (codes + per-output-channel scales [N]).  A Linear without codes runs in bf16.
+struct Linear {
+  const __nv_bfloat16* w = nullptr;
+  uint8_t* codes = nullptr;
+  float* scale = nullptr;
+};
+
+// The activation rows [M, K] a Linear reads: bf16 rows, and in the fp8 Linear mode their e4m3 codes + row scales [M]
+struct Act {
+  const __nv_bfloat16* rows = nullptr;
   uint8_t* codes = nullptr;
   float* scale = nullptr;
 };
 
 struct SubBlock {
-  const __nv_bfloat16 *wq = nullptr, *wk = nullptr, *wv = nullptr, *wo = nullptr;  // attention
-  const float *gq = nullptr, *gk = nullptr;                                        // RMSNorm gamma (f32 copy)
-  const __nv_bfloat16 *w1 = nullptr, *w2 = nullptr;                                // MLP
-  const __nv_bfloat16 *ada1 = nullptr, *ada2 = nullptr;                            // adaLN-LoRA
-  // fp8 Linear mode: FA to_q/to_k/to_v/to_out, CA to_q/to_out (q8, o8), MLP layer1/layer2 (l1, l2)
-  W8 q8, k8, v8, o8, l1, l2;
+  Linear q, k, v, o;                                    // attention to_q / to_k / to_v / to_out
+  const float *gq = nullptr, *gk = nullptr;             // RMSNorm gamma (f32 copy)
+  Linear l1, l2;                                        // MLP layer1 / layer2
+  const __nv_bfloat16 *ada1 = nullptr, *ada2 = nullptr;  // adaLN-LoRA
 };
+
+// The Linears of a block that run in e4m3 in the fp8 Linear mode, in their order inside h->w8: FA to_q / to_k / to_v /
+// to_out, CA to_q / to_out, MLP layer1 [F, D] and layer2 [D, F]; the others are [D, D].
+struct Fp8Linear {
+  int sub;  // 0 FA, 1 CA, 2 MLP
+  Linear SubBlock::*lin;
+  bool n_ffn, k_ffn;  // N, K is ffn_dim (else model_channels)
+  size_t n(const g3c_dit_config& c) const { return n_ffn ? c.ffn_dim : c.model_channels; }
+  size_t k(const g3c_dit_config& c) const { return k_ffn ? c.ffn_dim : c.model_channels; }
+};
+constexpr Fp8Linear kFp8Linears[] = {
+    {0, &SubBlock::q, false, false}, {0, &SubBlock::k, false, false}, {0, &SubBlock::v, false, false},
+    {0, &SubBlock::o, false, false}, {1, &SubBlock::q, false, false}, {1, &SubBlock::o, false, false},
+    {2, &SubBlock::l1, true, false}, {2, &SubBlock::l2, false, true}};
 
 }  // namespace g3c
 
@@ -234,25 +258,8 @@ static int prof_mark(g3c_dit* h, int cat, bool begin, cudaStream_t st) {
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
-// Layout of the fp8 weight copies inside h->w8: per block, the eight Linears in the order FA q, k, v, out, CA q, out,
-// MLP layer1, layer2, each as codes [N, K] then scales [N].  Returns the bytes; assigns the W8 pointers when blk is sized.
-static size_t fp8_layout(g3c_dit* h) {
-  const size_t D = h->cfg.model_channels, F = h->cfg.ffn_dim;
-  const size_t nk[8][2] = {{D, D}, {D, D}, {D, D}, {D, D}, {D, D}, {D, D}, {F, D}, {D, F}};
-  size_t off = 0;
-  for (int i = 0; i < h->cfg.num_blocks; ++i) {
-    for (int j = 0; j < 8; ++j) {
-      if (h->w8 && (int)h->blk.size() == h->cfg.num_blocks) {
-        SubBlock &fa = h->blk[i][0], &ca = h->blk[i][1], &mlp = h->blk[i][2];
-        W8* dst[8] = {&fa.q8, &fa.k8, &fa.v8, &fa.o8, &ca.q8, &ca.o8, &mlp.l1, &mlp.l2};
-        dst[j]->codes = (uint8_t*)h->w8 + off;
-        dst[j]->scale = (float*)((char*)h->w8 + off + align_up(nk[j][0] * nk[j][1], 1024));
-      }
-      off += align_up(nk[j][0] * nk[j][1], 1024) + align_up(nk[j][0] * 4, 1024);
-    }
-  }
-  return off;
-}
+// Bytes of one e4m3 copy inside h->w8: codes [N, K], then scales [N] from offset align_up(N * K, 1024)
+static size_t fp8_copy_bytes(size_t n, size_t k) { return align_up(n * k, 1024) + align_up(n * 4, 1024); }
 
 static int resolve(g3c_dit* h, cudaStream_t st) {
   if (h->resolved) return G3C_OK;
@@ -275,7 +282,7 @@ static int resolve(g3c_dit* h, cudaStream_t st) {
   TRY(need_bf16(h, "final_layer.linear.weight", {(int64_t)c.out_channels * 4, D}, &h->w_final));
   TRY(need_bf16(h, "final_layer.adaLN_modulation.1.weight", {R, D}, &h->f_ada1));
   TRY(need_bf16(h, "final_layer.adaLN_modulation.2.weight", {2 * D, R}, &h->f_ada2));
-  h->blk.resize(c.num_blocks);
+  h->blk.assign(c.num_blocks, std::array<SubBlock, 3>{});  // no e4m3 copies until the fp8 pass below
   if (!h->gammas) G3C_CUDA(cudaMalloc(&h->gammas, sizeof(float) * 128 * 4 * c.num_blocks));
   for (int i = 0; i < c.num_blocks; ++i) {
     for (int j = 0; j < 3; ++j) {
@@ -285,10 +292,10 @@ static int resolve(g3c_dit* h, cudaStream_t st) {
       TRY(need_bf16(h, p + "adaLN_modulation.2.weight", {3 * D, R}, &s.ada2));
       if (j < 2) {
         const int64_t kin = j == 0 ? D : C;
-        TRY(need_bf16(h, p + "block.attn.to_q.0.weight", {D, D}, &s.wq));
-        TRY(need_bf16(h, p + "block.attn.to_k.0.weight", {D, kin}, &s.wk));
-        TRY(need_bf16(h, p + "block.attn.to_v.0.weight", {D, kin}, &s.wv));
-        TRY(need_bf16(h, p + "block.attn.to_out.0.weight", {D, D}, &s.wo));
+        TRY(need_bf16(h, p + "block.attn.to_q.0.weight", {D, D}, &s.q.w));
+        TRY(need_bf16(h, p + "block.attn.to_k.0.weight", {D, kin}, &s.k.w));
+        TRY(need_bf16(h, p + "block.attn.to_v.0.weight", {D, kin}, &s.v.w));
+        TRY(need_bf16(h, p + "block.attn.to_out.0.weight", {D, D}, &s.o.w));
         const __nv_bfloat16 *gq = nullptr, *gk = nullptr;
         TRY(need_bf16(h, p + "block.attn.to_q.1.weight", {128}, &gq));
         TRY(need_bf16(h, p + "block.attn.to_k.1.weight", {128}, &gk));
@@ -301,22 +308,24 @@ static int resolve(g3c_dit* h, cudaStream_t st) {
         s.gq = dst;
         s.gk = dst + 128;
       } else {
-        TRY(need_bf16(h, p + "block.layer1.weight", {F, D}, &s.w1));
-        TRY(need_bf16(h, p + "block.layer2.weight", {D, F}, &s.w2));
+        TRY(need_bf16(h, p + "block.layer1.weight", {F, D}, &s.l1.w));
+        TRY(need_bf16(h, p + "block.layer2.weight", {D, F}, &s.l2.w));
       }
     }
   }
+  // fp8 Linear mode: (re)quantise every fp8 Linear from the registered weights into its slot of h->w8 (block after
+  // block, in the order of kFp8Linears).  Reached after g3c_dit_load and after enabling the mode.
   if (h->fp8) {
-    fp8_layout(h);
-    // (re)quantise every fp8 Linear from the registered weights: reached after g3c_dit_load and after enabling the mode
-    for (int i = 0; i < c.num_blocks; ++i) {
-      const SubBlock &fa = h->blk[i][0], &ca = h->blk[i][1], &mlp = h->blk[i][2];
-      const struct { const __nv_bfloat16* w; const W8& q; int64_t n, k; } lin[8] = {
-          {fa.wq, fa.q8, D, D}, {fa.wk, fa.k8, D, D}, {fa.wv, fa.v8, D, D}, {fa.wo, fa.o8, D, D},
-          {ca.wq, ca.q8, D, D}, {ca.wo, ca.o8, D, D}, {mlp.w1, mlp.l1, F, D}, {mlp.w2, mlp.l2, D, F}};
-      for (const auto& l : lin)
-        TRY(quant_rows_e4m3(l.w, (int)l.k, (int)l.n, (int)l.k, l.q.codes, (int)l.k, l.q.scale, st));
-    }
+    char* w8 = (char*)h->w8;
+    for (auto& b : h->blk)
+      for (const Fp8Linear& l : kFp8Linears) {
+        Linear& lin = b[l.sub].*l.lin;
+        const size_t n = l.n(c), k = l.k(c);
+        lin.codes = (uint8_t*)w8;
+        lin.scale = (float*)(w8 + align_up(n * k, 1024));
+        w8 += fp8_copy_bytes(n, k);
+        TRY(quant_rows_e4m3(lin.w, (int)k, (int)n, (int)k, lin.codes, (int)k, lin.scale, st));
+      }
   }
   h->resolved = true;
   return G3C_OK;
@@ -414,6 +423,27 @@ static int modulation(g3c_dit* h, float timestep, int& n, cudaStream_t st) {
   return G3C_OK;
 }
 
+// Every Linear of a block: out = epi(a . W^T) [M, N], or with vt = true its transpose W . a^T [N, M] (V^T).  It runs on
+// the e4m3 copy when the Linear has one, dequantising with both row scales before the epilogue, and on the bf16 weight
+// otherwise; `a` must carry codes exactly when the weight does.
+static int linear(const Linear& w, const Act& a, bool vt, int M, int N, int Kin, void* out, int epi, const float* gate,
+                  const NormRope* nr, cudaStream_t st) {
+  const bool f8 = w.codes != nullptr;
+  if (f8 != (a.codes != nullptr)) {
+    set_error("dit_forward: a Linear with%s e4m3 weights got activations with%s codes", f8 ? "" : "out", f8 ? "out" : "");
+    return G3C_ESTATE;
+  }
+  const void *A = f8 ? (const void*)a.codes : a.rows, *B = f8 ? (const void*)w.codes : w.w;
+  const float *sa = a.scale, *sb = w.scale;
+  if (vt) {
+    std::swap(A, B);
+    std::swap(sa, sb);
+    std::swap(M, N);
+  }
+  if (f8) return gemm_fp8(A, sa, B, sb, out, M, N, Kin, Kin, Kin, N, epi, gate, 0, st, nr);
+  return gemm_bf16(A, B, out, M, N, Kin, Kin, Kin, N, epi, gate, 0, st, nr);
+}
+
 static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const void* cond_pose,
                    const void* padding_mask, float timestep, const void* ctx, void* out,
                    cudaStream_t st) {
@@ -426,36 +456,37 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
   const int D = c.model_channels, F = c.ffn_dim, L = h->L, heads = c.num_heads;
   const int Lk_all = L * h->cp_size;
   const float attn_scale = 0.6931471805599453f;  // ln 2: 1/sqrt(128) * log2(e) is folded into the query RMSNorm gain
+  int n = 0;
+  // fp8 Linear mode (h->fp8): the Linears of kFp8Linears read e4m3 codes of their activation rows, xn from the fused
+  // LN-modulate (which then writes no bf16 xn), att and hid from a quantisation pass of their own.  K and V^T stay bf16,
+  // so the context-parallel exchange is the same in both modes.
+  Act xn{h->xn}, att{h->att}, hid{h->hid};
+  if (h->fp8) {
+    xn = {nullptr, h->xn8, h->xn8_s};
+    att = {h->att, h->att8, h->att8_s};
+    hid = {h->hid, h->hid8, h->hid8_s};
+  }
+  const Act ctx_rows{(const __nv_bfloat16*)ctx};
+  auto ln_mod = [&](const __nv_bfloat16* pos, const float* m) {
+    return xn.codes ? ln_modulate_e4m3(h->x, pos, m, m + D, xn.codes, xn.scale, L, D, 1e-6f, st)
+                    : ln_modulate(h->x, pos, m, m + D, h->xn, L, D, 1e-6f, st);
+  };
   // to_q / to_k: Linear + per-head RMSNorm (+ RoPE), fused into the GEMM epilogue: the norm and the rotation act on the
   // fp32 accumulators in registers, so the projection never round-trips [tokens, D] bf16 through a separate pass.
-  auto proj_norm_rope = [&](const void* a, const void* w, __nv_bfloat16* out, int M, int Kin, const float* gamma,
+  auto proj_norm_rope = [&](const Linear& w, const Act& a, int M, int Kin, __nv_bfloat16* out, const float* gamma,
                             const float* cs) {
     NormRope nr;
     nr.gamma = gamma;
     nr.cs = cs;
     nr.eps = 1e-6f;
-    return gemm_bf16(a, w, out, M, D, Kin, Kin, Kin, D, G3C_EPI_BF16, nullptr, 0, st, &nr);
+    return linear(w, a, false, M, D, Kin, out, G3C_EPI_BF16, nullptr, &nr, st);
   };
-  // fp8 Linear mode (h->fp8): the eight large Linears of a block read e4m3 codes of their activation rows (xn8 from the
-  // fused LN-modulate, att8 / hid8 from a quantisation pass) and the engine's e4m3 weight copies; the GEMM dequantises
-  // with both row scales before its epilogue.  K and V^T stay bf16, so the context-parallel exchange is unchanged.
-  const bool f8 = h->fp8;
-  auto ln_mod = [&](const __nv_bfloat16* pos, const float* m) {
-    return f8 ? ln_modulate_e4m3(h->x, pos, m, m + D, h->xn8, h->xn8_s, L, D, 1e-6f, st)
-              : ln_modulate(h->x, pos, m, m + D, h->xn, L, D, 1e-6f, st);
+  // x += gate * (a . W^T): the gated-residual output projection, after the pass that quantises a when it feeds codes
+  auto out_proj = [&](const Linear& w, const Act& a, int Kin, const float* gate) -> int {
+    if (a.codes) K(CAT_ELTWISE, quant_rows_e4m3(a.rows, Kin, L, Kin, a.codes, Kin, a.scale, st));
+    K(CAT_GEMM, linear(w, a, false, L, D, Kin, h->x, G3C_EPI_GATED_RESIDUAL_F32, gate, nullptr, st));
+    return G3C_OK;
   };
-  auto proj8_norm_rope = [&](const W8& w, __nv_bfloat16* out, const float* gamma, const float* cs) {
-    NormRope nr;
-    nr.gamma = gamma;
-    nr.cs = cs;
-    nr.eps = 1e-6f;
-    return gemm_fp8(h->xn8, h->xn8_s, w.codes, w.scale, out, L, D, D, D, D, D, G3C_EPI_BF16, nullptr, 0, st, &nr);
-  };
-  // x += gate * (a8 . w^T), a8 = codes [L, Kin] of att (Kin = D) or hid (Kin = F)
-  auto out8 = [&](const uint8_t* a8, const float* sa, const W8& w, int Kin, const float* gate) {
-    return gemm_fp8(a8, sa, w.codes, w.scale, h->x, L, D, Kin, Kin, Kin, D, G3C_EPI_GATED_RESIDUAL_F32, gate, 0, st);
-  };
-  int n = 0;
 
   // ---- input assembly + patch embedding (general_dit_video_conditioned.py:112-118,
   //      general_dit.py:304-311, blocks.py:153-163)
@@ -470,38 +501,33 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
   // ---- timestep embedding + adaLN-LoRA modulation vectors (cached per timestep)
   TRY(modulation(h, timestep, n, st));
 
-  __nv_bfloat16* k_loc = h->k_all + (size_t)h->cp_rank * L * D;
-  __nv_bfloat16* vt_loc = h->vt_all + (size_t)h->cp_rank * L * D;
-
+  const bool p2p = h->cp_size > 1 && h->cp_p2p;
   for (int i = 0; i < c.num_blocks; ++i) {
     // ---------------- FA: full self-attention (blocks.py:455-463, attention.py:247-289)
     {
       const SubBlock& s = h->blk[i][0];
       const float* m = h->mods + (size_t)(i * 3 + 0) * 3 * D;
       K(CAT_ELTWISE, ln_mod(h->pos, m));   // + abs-pos add
-      if (h->cp_size > 1 && h->cp_p2p) {
+      // K and V^T of every rank, [cp][L, D] and [cp][D][L]: in p2p mode one of the two layer-parity sets of the
+      // peer-mapped region, else k_all / vt_all.  This rank projects its slice straight into it.
+      if (p2p) G3C_REQUIRE(h->peers_open, "dit_forward: context-parallel peers not imported (g3c_dit_cp_import)");
+      const uint32_t seq = p2p ? ++h->kv_seq : 0;
+      const int set = seq & 1, me = h->cp_rank;
+      char* reg = (char*)h->cp_region;
+      __nv_bfloat16* kb = p2p ? (__nv_bfloat16*)(reg + h->off_k[set]) : h->k_all;
+      __nv_bfloat16* vb = p2p ? (__nv_bfloat16*)(reg + h->off_vt[set]) : h->vt_all;
+      __nv_bfloat16* kl = kb + (size_t)me * L * D;
+      __nv_bfloat16* vl = vb + (size_t)me * L * D;
+      K(CAT_GEMM, proj_norm_rope(s.k, xn, L, D, kl, s.gk, h->rope));
+      K(CAT_GEMM, linear(s.v, xn, true, L, D, D, vl, G3C_EPI_BF16, nullptr, nullptr, st));  // V^T
+      if (p2p) {
         // all-gather through peer memory: every rank produces its K / V^T slice locally, then the copy engines push
         // it into every peer's buffer on a side stream and raise a flag there, while this stream already runs the Q
         // projection and attention over the local chunk; attention picks up the remote chunks as their flags arrive.
         // Peer (me-1) is served first, then (me-2), ...: rank c consumes chunk c+1 first, so its k-th remote chunk is
         // the k-th push of its producer.  The flag that opens the chunk on a peer follows that peer's two copies on the
         // same stream (a 4-byte copy from a pinned ring: no kernel, see seq_ring).
-        G3C_REQUIRE(h->peers_open, "dit_forward: context-parallel peers not imported (g3c_dit_cp_import)");
-        const uint32_t seq = ++h->kv_seq;
-        const int set = seq & 1, me = h->cp_rank;
         const size_t slice = (size_t)L * D * 2;
-        char* reg = (char*)h->cp_region;
-        __nv_bfloat16* kb = (__nv_bfloat16*)(reg + h->off_k[set]);
-        __nv_bfloat16* vb = (__nv_bfloat16*)(reg + h->off_vt[set]);
-        __nv_bfloat16* kl = kb + (size_t)me * L * D;
-        __nv_bfloat16* vl = vb + (size_t)me * L * D;
-        if (f8) {
-          K(CAT_GEMM, proj8_norm_rope(s.k8, kl, s.gk, h->rope));
-          K(CAT_GEMM, gemm_fp8(s.v8.codes, s.v8.scale, h->xn8, h->xn8_s, vl, D, L, D, D, D, L, G3C_EPI_BF16, nullptr, 0, st));
-        } else {
-          K(CAT_GEMM, proj_norm_rope(h->xn, s.wk, kl, L, D, s.gk, h->rope));
-          K(CAT_GEMM, gemm_bf16(s.wv, h->xn, vl, D, L, D, D, D, L, G3C_EPI_BF16, nullptr, 0, st));  // V^T
-        }
         G3C_CUDA(cudaEventRecord(h->ev_kv, st));
         G3C_CUDA(cudaStreamWaitEvent(h->comm_stream, h->ev_kv, 0));
         uint32_t* slot = h->seq_ring + (seq % g3c_dit::kSeqRing);
@@ -516,46 +542,31 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
           G3C_CUDA(cudaMemcpyAsync(pb + h->off_flags + (size_t)(set * 8 + me) * 4, slot, 4, cudaMemcpyHostToDevice,
                                    h->comm_stream));
         }
-        if (f8) K(CAT_GEMM, proj8_norm_rope(s.q8, h->q, s.gq, h->rope));
-        else K(CAT_GEMM, proj_norm_rope(h->xn, s.wq, h->q, L, D, s.gq, h->rope));
-        ChunkGate gate;
+      } else if (h->cp_size > 1) {
+        // baseline mode (G3C_CP_MODE=nccl): one in-place all-gather of K and of V^T per layer on a side stream
+        G3C_CUDA(cudaEventRecord(h->ev_kv, st));
+        G3C_CUDA(cudaStreamWaitEvent(h->comm_stream, h->ev_kv, 0));
+        G3C_NCCL(nccl().GroupStart());
+        G3C_NCCL(nccl().AllGather(kl, h->k_all, (size_t)L * D, kNcclBfloat16, h->comm, h->comm_stream));
+        G3C_NCCL(nccl().AllGather(vl, h->vt_all, (size_t)L * D, kNcclBfloat16, h->comm, h->comm_stream));
+        G3C_NCCL(nccl().GroupEnd());
+        G3C_CUDA(cudaEventRecord(h->ev_gathered, h->comm_stream));
+        n += 2;
+      }
+      K(CAT_GEMM, proj_norm_rope(s.q, xn, L, D, h->q, s.gq, h->rope));
+      ChunkGate gate;
+      if (p2p) {
         gate.flags = (const uint32_t*)(reg + h->off_flags) + set * 8;
         gate.seq = seq;
         gate.first = me;
         gate.wait_ns = h->prof ? h->wait_ns : nullptr;
         h->wait_cta_launches = (double)((L + ATT_ROWS_PER_CTA - 1) / ATT_ROWS_PER_CTA) * heads;  // CTAs of one gated launch
-        K(CAT_ATTN_SELF, attn_fwd(h->q, kb, vb, h->att, L, Lk_all, heads, D, D, D, L, attn_scale, st, &gate));
-      } else {
-        if (f8) {
-          K(CAT_GEMM, proj8_norm_rope(s.k8, k_loc, s.gk, h->rope));
-          K(CAT_GEMM, gemm_fp8(s.v8.codes, s.v8.scale, h->xn8, h->xn8_s, vt_loc, D, L, D, D, D, L, G3C_EPI_BF16, nullptr,
-                               0, st));
-        } else {
-          K(CAT_GEMM, proj_norm_rope(h->xn, s.wk, k_loc, L, D, s.gk, h->rope));
-          K(CAT_GEMM, gemm_bf16(s.wv, h->xn, vt_loc, D, L, D, D, D, L, G3C_EPI_BF16, nullptr, 0, st));  // V^T
-        }
-        if (h->cp_size > 1) {
-          // baseline mode (G3C_CP_MODE=nccl): one in-place all-gather of K and of V^T per layer on a side stream
-          G3C_CUDA(cudaEventRecord(h->ev_kv, st));
-          G3C_CUDA(cudaStreamWaitEvent(h->comm_stream, h->ev_kv, 0));
-          G3C_NCCL(nccl().GroupStart());
-          G3C_NCCL(nccl().AllGather(k_loc, h->k_all, (size_t)L * D, kNcclBfloat16, h->comm, h->comm_stream));
-          G3C_NCCL(nccl().AllGather(vt_loc, h->vt_all, (size_t)L * D, kNcclBfloat16, h->comm, h->comm_stream));
-          G3C_NCCL(nccl().GroupEnd());
-          G3C_CUDA(cudaEventRecord(h->ev_gathered, h->comm_stream));
-          n += 2;
-        }
-        if (f8) K(CAT_GEMM, proj8_norm_rope(s.q8, h->q, s.gq, h->rope));
-        else K(CAT_GEMM, proj_norm_rope(h->xn, s.wq, h->q, L, D, s.gq, h->rope));
-        if (h->cp_size > 1) G3C_CUDA(cudaStreamWaitEvent(st, h->ev_gathered, 0));
-        K(CAT_ATTN_SELF, attn_fwd(h->q, h->k_all, h->vt_all, h->att, L, Lk_all, heads, D, D, D, L, attn_scale, st));
+      } else if (h->cp_size > 1) {
+        G3C_CUDA(cudaStreamWaitEvent(st, h->ev_gathered, 0));
       }
-      if (f8) {
-        K(CAT_ELTWISE, quant_rows_e4m3(h->att, D, L, D, h->att8, D, h->att8_s, st));
-        K(CAT_GEMM, out8(h->att8, h->att8_s, s.o8, D, m + 2 * D));
-      } else {
-        K(CAT_GEMM, gemm_bf16(h->att, s.wo, h->x, L, D, D, D, D, D, G3C_EPI_GATED_RESIDUAL_F32, m + 2 * D, 0, st));
-      }
+      K(CAT_ATTN_SELF,
+        attn_fwd(h->q, kb, vb, h->att, L, Lk_all, heads, D, D, D, L, attn_scale, st, p2p ? &gate : nullptr));
+      TRY(out_proj(s.o, att, D, m + 2 * D));
     }
     // ---------------- CA: cross-attention to the T5 context (blocks.py:464-471)
     {
@@ -563,32 +574,19 @@ static int forward(g3c_dit* h, const void* x_in, const void* cond_mask, const vo
       const float* m = h->mods + (size_t)(i * 3 + 1) * 3 * D;
       const int C = c.context_dim, M = h->ctx_len;
       K(CAT_ELTWISE, ln_mod(nullptr, m));
-      K(CAT_GEMM, proj_norm_rope(ctx, s.wk, h->kc, M, C, s.gk, nullptr));
-      K(CAT_GEMM, gemm_bf16(s.wv, ctx, h->vtc, D, M, C, C, C, M, G3C_EPI_BF16, nullptr, 0, st));
-      if (f8) K(CAT_GEMM, proj8_norm_rope(s.q8, h->q, s.gq, nullptr));
-      else K(CAT_GEMM, proj_norm_rope(h->xn, s.wq, h->q, L, D, s.gq, nullptr));
+      K(CAT_GEMM, proj_norm_rope(s.k, ctx_rows, M, C, h->kc, s.gk, nullptr));
+      K(CAT_GEMM, linear(s.v, ctx_rows, true, M, D, C, h->vtc, G3C_EPI_BF16, nullptr, nullptr, st));  // V^T
+      K(CAT_GEMM, proj_norm_rope(s.q, xn, L, D, h->q, s.gq, nullptr));
       K(CAT_ATTN_CROSS, attn_fwd(h->q, h->kc, h->vtc, h->att, L, M, heads, D, D, D, M, attn_scale, st));
-      if (f8) {
-        K(CAT_ELTWISE, quant_rows_e4m3(h->att, D, L, D, h->att8, D, h->att8_s, st));
-        K(CAT_GEMM, out8(h->att8, h->att8_s, s.o8, D, m + 2 * D));
-      } else {
-        K(CAT_GEMM, gemm_bf16(h->att, s.wo, h->x, L, D, D, D, D, D, G3C_EPI_GATED_RESIDUAL_F32, m + 2 * D, 0, st));
-      }
+      TRY(out_proj(s.o, att, D, m + 2 * D));
     }
     // ---------------- MLP (attention.py:91-102)
     {
       const SubBlock& s = h->blk[i][2];
       const float* m = h->mods + (size_t)(i * 3 + 2) * 3 * D;
       K(CAT_ELTWISE, ln_mod(nullptr, m));
-      if (f8) {
-        K(CAT_GEMM, gemm_fp8(h->xn8, h->xn8_s, s.l1.codes, s.l1.scale, h->hid, L, F, D, D, D, F, G3C_EPI_GELU_BF16,
-                             nullptr, 0, st));
-        K(CAT_ELTWISE, quant_rows_e4m3(h->hid, F, L, F, h->hid8, F, h->hid8_s, st));
-        K(CAT_GEMM, out8(h->hid8, h->hid8_s, s.l2, F, m + 2 * D));
-      } else {
-        K(CAT_GEMM, gemm_bf16(h->xn, s.w1, h->hid, L, F, D, D, D, F, G3C_EPI_GELU_BF16, nullptr, 0, st));
-        K(CAT_GEMM, gemm_bf16(h->hid, s.w2, h->x, L, D, F, F, F, D, G3C_EPI_GATED_RESIDUAL_F32, m + 2 * D, 0, st));
-      }
+      K(CAT_GEMM, linear(s.l1, xn, false, L, F, D, h->hid, G3C_EPI_GELU_BF16, nullptr, nullptr, st));
+      TRY(out_proj(s.l2, hid, F, m + 2 * D));
     }
   }
   // ---- final layer + unpatchify (blocks.py:222-242, general_dit.py:328-358)
@@ -930,7 +928,8 @@ int g3c_dit_set_linear_fp8(g3c_dit_t* h, int on) {
   if ((on != 0) == h->fp8) return G3C_OK;
   free_ws(h);  // the fp8 activation buffers come and go with the shape's workspace
   if (on) {
-    const size_t bytes = fp8_layout(h);
+    size_t bytes = 0;
+    for (const Fp8Linear& l : kFp8Linears) bytes += h->cfg.num_blocks * fp8_copy_bytes(l.n(h->cfg), l.k(h->cfg));
     cudaError_t e = cudaMalloc(&h->w8, bytes);
     if (e != cudaSuccess) {
       h->w8 = nullptr;
@@ -943,11 +942,9 @@ int g3c_dit_set_linear_fp8(g3c_dit_t* h, int on) {
     G3C_CUDA(cudaFree(h->w8));
     h->w8 = nullptr;
     h->w8_bytes = 0;
-    for (auto& b : h->blk)
-      for (auto& sb : b) sb.q8 = sb.k8 = sb.v8 = sb.o8 = sb.l1 = sb.l2 = W8();
   }
   h->fp8 = on != 0;
-  h->resolved = false;  // resolve() quantises the weights into the new copies
+  h->resolved = false;  // resolve() points the Linears at the new copies and quantises into them, or drops the old ones
   return G3C_OK;
 }
 
