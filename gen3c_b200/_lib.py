@@ -116,6 +116,7 @@ SIGNATURES = {
     "g3c_dit_last_launch_count": (_I, [_P]),
     "g3c_dit_read_tables": (_I, [_P, _I, _P, _P, _P]),
     "g3c_dit_read_modulation": (_I, [_P, _F, _P, _P, _P]),
+    "g3c_dit_read_step": (_I, [_P, _P, _P, _P, _P, _P]),
 }
 
 _lib = None

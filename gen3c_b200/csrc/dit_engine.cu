@@ -170,6 +170,9 @@ struct g3c_dit {
   float *rope = nullptr, *yfin = nullptr, *mods = nullptr, *modf = nullptr, *vec_s = nullptr,
         *vec_emb = nullptr, *vec_h1 = nullptr, *vec_lora = nullptr, *vec_a = nullptr, *freqs = nullptr;
   __nv_bfloat16 *lat_xtilde = nullptr, *lat_xin = nullptr, *lat_oc = nullptr, *lat_ou = nullptr;
+  // the cond / uncond outputs the last denoise step's sampler_post read (lat_oc / lat_ou, or the CFG exchange region);
+  // NULL until a step completes after g3c_dit_set_shape or g3c_dit_set_linear_fp8 (g3c_dit_read_step)
+  const __nv_bfloat16 *step_oc = nullptr, *step_ou = nullptr;
   // fp8 Linear mode: e4m3 codes + row scales of the GEMM A operands (xn, att, hid)
   uint8_t *xn8 = nullptr, *att8 = nullptr, *hid8 = nullptr;
   float *xn8_s = nullptr, *att8_s = nullptr, *hid8_s = nullptr;
@@ -643,6 +646,7 @@ static void free_ws(g3c_dit* h) {
   h->L = 0;
   h->tables_ready = false;
   h->mods_valid = false;
+  h->step_oc = h->step_ou = nullptr;
 }
 
 int g3c_dit_destroy(g3c_dit_t* h) {
@@ -758,6 +762,7 @@ int g3c_dit_disable_cp(g3c_dit_t* h) {
 
 int g3c_dit_set_shape(g3c_dit_t* h, int T_local, int H_latent, int W_latent, int ctx_len, float fps) {
   G3C_REQUIRE(h, "set_shape: null handle");
+  h->step_oc = h->step_ou = nullptr;
   const g3c_dit_config& c = h->cfg;
   G3C_REQUIRE(T_local > 0 && H_latent > 0 && W_latent > 0 && H_latent % 2 == 0 && W_latent % 2 == 0,
               "set_shape: latent H, W must be positive and even (patch 2)");
@@ -872,6 +877,7 @@ int g3c_denoise_step(g3c_dit_t* h, const g3c_step_args* a, void* stream) {
               "denoise_step: null argument");
   G3C_REQUIRE(h->L > 0, "denoise_step: g3c_dit_set_shape was not called");
   G3C_REQUIRE(a->sigma > 0, "denoise_step: sigma must be positive");
+  h->step_oc = h->step_ou = nullptr;
   cudaStream_t st = (cudaStream_t)stream;
   const size_t plane = (size_t)h->Hl * h->Wl;
   // t = 0.25 * ln(sigma)  (EDMEulerScheduler timesteps; model_v2w.py:131-140)
@@ -919,12 +925,15 @@ int g3c_denoise_step(g3c_dit_t* h, const g3c_step_args* a, void* stream) {
                    a->guidance, a->sigma, a->sigma_next, a->sigma_aug, a->sigma_data, (__nv_bfloat16*)a->xt_next,
                    (__nv_bfloat16*)a->net_output, st));
   h->launches = n_launch;
+  h->step_oc = oc;
+  h->step_ou = ou;
   return G3C_OK;
 }
 
 int g3c_dit_set_linear_fp8(g3c_dit_t* h, int on) {
   G3C_REQUIRE(h, "set_linear_fp8: null handle");
   G3C_REQUIRE(h->cfg.ffn_dim % 16 == 0, "set_linear_fp8: ffn_dim=%d must be a multiple of 16", h->cfg.ffn_dim);
+  h->step_oc = h->step_ou = nullptr;
   if ((on != 0) == h->fp8) return G3C_OK;
   free_ws(h);  // the fp8 activation buffers come and go with the shape's workspace
   if (on) {
@@ -1039,6 +1048,21 @@ int g3c_dit_read_modulation(g3c_dit_t* h, float timestep, float* mods, float* mo
   G3C_CUDA(cudaMemcpyAsync(mods, h->mods, (size_t)h->cfg.num_blocks * 3 * 3 * D * sizeof(float),
                            cudaMemcpyDeviceToDevice, st));
   G3C_CUDA(cudaMemcpyAsync(modf, h->modf, 2 * D * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return G3C_OK;
+}
+
+int g3c_dit_read_step(g3c_dit_t* h, void* xtilde, void* xin, void* oc, void* ou, void* stream) {
+  G3C_REQUIRE(h && xtilde && xin && oc && ou, "dit_read_step: null argument");
+  if (!h->step_oc) {
+    set_error("dit_read_step: no g3c_denoise_step since the last g3c_dit_set_shape or g3c_dit_set_linear_fp8");
+    return G3C_ESTATE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t bytes = (size_t)16 * h->T * h->Hl * h->Wl * sizeof(__nv_bfloat16);
+  G3C_CUDA(cudaMemcpyAsync(xtilde, h->lat_xtilde, bytes, cudaMemcpyDeviceToDevice, st));
+  G3C_CUDA(cudaMemcpyAsync(xin, h->lat_xin, bytes, cudaMemcpyDeviceToDevice, st));
+  G3C_CUDA(cudaMemcpyAsync(oc, h->step_oc, bytes, cudaMemcpyDeviceToDevice, st));
+  G3C_CUDA(cudaMemcpyAsync(ou, h->step_ou, bytes, cudaMemcpyDeviceToDevice, st));
   return G3C_OK;
 }
 

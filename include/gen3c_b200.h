@@ -330,6 +330,10 @@ int g3c_dit_read_tables(g3c_dit_t* h, int t0, float* rope, void* pos, void* stre
  * block i, sub-block j at row i*3 + j), modf f32 [2D] (final layer shift | scale).  Goes through the forward's
  * per-timestep cache (a forward right after at the same timestep reuses the vectors). */
 int g3c_dit_read_modulation(g3c_dit_t* h, float timestep, float* mods, float* modf, void* stream);
+/* The four bf16 [16,T,H,W] latents of the last g3c_denoise_step: x~ and x_in as sampler_pre wrote them, and the cond /
+ * uncond network outputs sampler_post read (under CFG parallelism one of them is the partner's copy in the exchange
+ * region).  G3C_ESTATE when no step has completed since the last g3c_dit_set_shape or g3c_dit_set_linear_fp8. */
+int g3c_dit_read_step(g3c_dit_t* h, void* xtilde, void* xin, void* oc, void* ou, void* stream);
 
 #ifdef __cplusplus
 }
