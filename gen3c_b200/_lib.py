@@ -117,6 +117,7 @@ SIGNATURES = {
     "g3c_dit_read_tables": (_I, [_P, _I, _P, _P, _P]),
     "g3c_dit_read_modulation": (_I, [_P, _F, _P, _P, _P]),
     "g3c_dit_read_step": (_I, [_P, _P, _P, _P, _P, _P]),
+    "g3c_attn_fwd_gated": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _F, _P, C.c_uint32, _I, _P, _P]),
 }
 
 _lib = None

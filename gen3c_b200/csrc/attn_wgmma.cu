@@ -547,6 +547,17 @@ extern "C" int g3c_attn_fwd(const void* q, const void* k, const void* vt, void* 
                        (cudaStream_t)stream, nullptr);
 }
 
+extern "C" int g3c_attn_fwd_gated(const void* q, const void* k, const void* vt, void* o, int Lq, int Lk, int heads,
+                                  int ldq, int ldk, int ldo, int vt_chunk_len, float scale, const uint32_t* flags,
+                                  uint32_t seq, int first, unsigned long long* wait_ns, void* stream) {
+  g3c::ChunkGate gate;
+  gate.flags = flags;
+  gate.seq = seq;
+  gate.first = first;
+  gate.wait_ns = wait_ns;
+  return g3c::attn_fwd(q, k, vt, o, Lq, Lk, heads, ldq, ldk, ldo, vt_chunk_len, scale, (cudaStream_t)stream, &gate);
+}
+
 extern "C" int g3c_attn_fwd_sbhd(const void* q, const void* k, const void* v, void* o, int Lq, int Lk, int batch,
                                  int heads, int ldq, int ldk, int ldv, int ldo, float scale, void* stream) {
   return g3c::attn_fwd_sbhd(q, k, v, o, Lq, Lk, batch, heads, ldq, ldk, ldv, ldo, scale, (cudaStream_t)stream);

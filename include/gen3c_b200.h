@@ -334,6 +334,15 @@ int g3c_dit_read_modulation(g3c_dit_t* h, float timestep, float* mods, float* mo
  * uncond network outputs sampler_post read (under CFG parallelism one of them is the partner's copy in the exchange
  * region).  G3C_ESTATE when no step has completed since the last g3c_dit_set_shape or g3c_dit_set_linear_fp8. */
 int g3c_dit_read_step(g3c_dit_t* h, void* xtilde, void* xin, void* oc, void* ou, void* stream);
+/* g3c_attn_fwd with the context-parallel chunk gate of the engine's peer-memory mode: the KV tiles are visited chunk by
+ * chunk (chunks of vt_chunk_len keys, in K and in V^T) starting with chunk `first`, and the TMA loader of each CTA reads
+ * a chunk c != first only once flags[c] >= seq (a system-scope acquire; flags is device memory of Lk / vt_chunk_len
+ * uint32, typically raised by a copy after the chunk's data).  The local chunk `first` is never gated.  wait_ns (device,
+ * optional): += ns each CTA's loader spent polling.  A flag that stays below seq traps the kernel after the peer timeout
+ * (G3C_PEER_TIMEOUT_S, 600 s). */
+int g3c_attn_fwd_gated(const void* q, const void* k, const void* vt, void* o, int Lq, int Lk, int heads,
+                       int ldq, int ldk, int ldo, int vt_chunk_len, float scale,
+                       const uint32_t* flags, uint32_t seq, int first, unsigned long long* wait_ns, void* stream);
 
 #ifdef __cplusplus
 }

@@ -3,11 +3,13 @@ row max m moves, and O and the row sums are rescaled, only when some row of a wa
 log2 units; otherwise the tile is exponentiated against the stale m, so P <= 2^8.  Each test builds scores whose row
 maxima are known exactly (scale = ln 2: S is in log2 units), runs both V layouts (V^T through g3c_attn_fwd,
 token-major V through g3c_attn_fwd_sbhd) and compares with an fp64 softmax.  With Lk a multiple of 128 the two layouts
-must also agree bit for bit."""
+must also agree bit for bit.  Both outputs also pass the float64 checks of tests/attn_ref64.py."""
 import math
 
 import pytest
 import torch
+
+from tests import attn_ref64
 
 pytestmark = pytest.mark.gpu
 
@@ -49,6 +51,7 @@ def check(q, k, v, heads=1):
             continue
         assert torch.isfinite(o.float()).all()
         assert rel(o, want) < TOL, rel(o, want)
+        attn_ref64.check(o, q, k, v, heads, LN2)
     if o_vt is not None:
         assert torch.equal(o_vt, o_tok)
 
@@ -121,3 +124,4 @@ def test_masked_tail_with_jump(Lk):
     _, o = run_both(q, k, v, 1)
     assert torch.isfinite(o.float()).all()
     assert rel(o, want) < TOL, rel(o, want)
+    attn_ref64.check(o, q, k, v, 1, LN2)

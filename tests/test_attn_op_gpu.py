@@ -8,6 +8,8 @@ import os
 import pytest
 import torch
 
+from tests import attn_ref64
+
 pytestmark = pytest.mark.gpu
 
 TOL = 5e-3
@@ -29,6 +31,13 @@ def ref(q, k, v, scale=128 ** -0.5):
     o = torch.nn.functional.scaled_dot_product_attention(qq, kk, vv, scale=scale)
     s, b, h, d = q.shape
     return o.permute(2, 0, 1, 3).reshape(s, b, h * d)
+
+
+def check64(o, q, k, v, scale=128 ** -0.5, label=""):
+    """both float64 checks of tests/attn_ref64.py on sbhd tensors (batch x heads = the kernel's heads)"""
+    s, b, h, _ = q.shape
+    attn_ref64.check(o.reshape(s, -1), q.reshape(s, -1), k.reshape(k.shape[0], -1), v.reshape(v.shape[0], -1), b * h,
+                     scale, label=label)
 
 
 def op(h, **kw):
@@ -61,14 +70,17 @@ def test_parity_with_sdpa(Lk, Lq, b, h, log2_units):
     exponentiates S directly)."""
     q, k, v = sbhd(Lq, b, h, seed=Lk + Lq), sbhd(Lk, b, h, seed=2 * Lk + 1), sbhd(Lk, b, h, seed=3 * Lk + 2)
     want = ref(q, k, v)
+    scale = 128 ** -0.5
     if log2_units:
         q = (q.float() * (128 ** -0.5 * math.log2(math.e))).to(torch.bfloat16)
         want = ref(q, k, v, scale=math.log(2.0))
-        o = op(h, softmax_scale=math.log(2.0))(q, k, v)
+        scale = math.log(2.0)
+        o = op(h, softmax_scale=scale)(q, k, v)
     else:
         o = op(h)(q, k, v)
     assert o.shape == (Lq, b, h * 128)
     assert rel(o, want) < TOL, rel(o, want)
+    check64(o, q, k, v, scale, label=f"Lk={Lk} Lq={Lq} b={b} h={h} log2={log2_units}")
 
 
 @pytest.mark.parametrize("Lq,Lk,h", [(300, 128, 2), (1000, 1024, 2), (77, 7040, 1), (56320, 56320, 32)])
@@ -104,6 +116,7 @@ def test_tail_mask_negative_control(Lk):
     assert rel(with_zero_keys, want) >= 10 * TOL
     o = op(h)(q, k, v)
     assert rel(o, want) < TOL, rel(o, want)
+    check64(o, q, k, v)
 
 
 @pytest.mark.parametrize("Lk,first", [(100, 40), (1000, 950)])
@@ -118,6 +131,7 @@ def test_score_jump_in_partial_last_tile(Lk, first):
     o = op(h)(q, k, v)
     assert torch.isfinite(o.float()).all()
     assert rel(o, want) < TOL, rel(o, want)
+    check64(o, q, k, v)
 
 
 def test_batch_isolation():
@@ -130,6 +144,7 @@ def test_batch_isolation():
     o1 = op(h)(q[:, :1], k[:, :1], v[:, :1])
     assert torch.equal(o2[:, 0], o1[:, 0])
     assert rel(o2, ref(q, k, v)) < TOL
+    check64(o2, q, k, v)
 
 
 def test_errors():

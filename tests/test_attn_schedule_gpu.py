@@ -5,6 +5,8 @@ full-width launch (a ring stage reused too early would make repeated launches di
 import pytest
 import torch
 
+from tests import attn_ref64
+
 pytestmark = pytest.mark.gpu
 
 
@@ -27,13 +29,16 @@ def sdpa_ref(q, k, v, heads):
 
 
 def run(Lq, Lk, heads, chunks, seed):
+    """(o, fp32 reference); o also passes both float64 checks of tests/attn_ref64.py"""
     from gen3c_b200 import ops
 
     D = heads * 128
     q, k, v = bf(Lq, D, seed=seed), bf(Lk, D, seed=seed + 1), bf(Lk, D, seed=seed + 2)
     cl = Lk // chunks
     vt = v.reshape(chunks, cl, D).permute(0, 2, 1).contiguous()  # [chunks, D, chunk_len]
-    return ops.attention(q, k, vt, heads, vt_chunk_len=cl), sdpa_ref(q, k, v, heads)
+    o = ops.attention(q, k, vt, heads, vt_chunk_len=cl)
+    attn_ref64.check(o, q, k, v, heads, 128 ** -0.5, label=f"Lq={Lq} Lk={Lk} chunks={chunks}")
+    return o, sdpa_ref(q, k, v, heads)
 
 
 @pytest.mark.parametrize("n_kv", [2, 3, 5, 6])
@@ -59,7 +64,8 @@ def test_chunk_boundaries_mid_ring():
 
 def test_full_width_repeat_is_bit_identical():
     """Full self-attention width (56 320 keys, 440 KV tiles), 2 heads: the schedule is deterministic, so a second launch
-    must reproduce the first exactly; the first is also checked against the fp32 reference on a subset of query rows."""
+    must reproduce the first exactly; the first is also checked against the fp32 reference and the float64 checks of
+    tests/attn_ref64.py on a subset of query rows."""
     from gen3c_b200 import ops
 
     L, heads = 56320, 2
@@ -73,3 +79,4 @@ def test_full_width_repeat_is_bit_identical():
     rows = torch.arange(0, L, 97, device="cuda")
     ref = sdpa_ref(q[rows], k, v, heads)
     assert rel(o1[rows], ref) < 5e-3, rel(o1[rows], ref)
+    attn_ref64.check(o1, q, k, v, heads, 128 ** -0.5, rows=rows, label="full width")

@@ -4,6 +4,8 @@ GEMM linearity and sampled-row agreement, LayerNorm-modulate statistics.  All th
 import pytest
 import torch
 
+from tests import attn_ref64
+
 pytestmark = pytest.mark.gpu
 
 L_FULL, HEADS = 56320, 32
@@ -21,7 +23,8 @@ def rel(a, b):
 def test_attention_full_size_rows_sum_to_one_and_match_reference_rows():
     """Lq = Lk = 56 320, 4 heads (enough to fill the GPU; every head runs the same code path):
     (1) V = 1 -> O = 1 exactly up to bf16 rounding (checks the running-max / row-sum bookkeeping over 440 KV tiles);
-    (2) 64 sampled query rows against an fp32 softmax(QK^T)V reference."""
+    (2) 64 sampled query rows against an fp32 softmax(QK^T)V reference, and 256 against both float64 checks of
+    tests/attn_ref64.py (every head)."""
     from gen3c_b200 import ops
 
     H = 4
@@ -38,6 +41,8 @@ def test_attention_full_size_rows_sum_to_one_and_match_reference_rows():
         s = (q[rows, sl].float() @ k[:, sl].float().T) * 128 ** -0.5
         ref = torch.softmax(s, dim=-1) @ v[:, sl].float()
         assert rel(o[rows, sl], ref) < 5e-3
+    rows64 = torch.randint(0, L_FULL, (256,), device="cuda", generator=torch.Generator(device="cuda").manual_seed(9))
+    attn_ref64.check(o, q, k, v, H, 128 ** -0.5, rows=rows64, label="full size")
 
 
 def test_attention_key_permutation_invariance():
@@ -49,6 +54,10 @@ def test_attention_key_permutation_invariance():
     a = ops.attention(q, k, v.T.contiguous(), H)
     b = ops.attention(q, k[perm].contiguous(), v[perm].T.contiguous(), H)
     assert rel(a, b) < 4e-3  # only the accumulation order and bf16 rounding of P differ
+    rows = torch.arange(0, Lq, 4, device="cuda")
+    ref = attn_ref64.Reference(q, k, v, H, 128 ** -0.5, rows)
+    ref.check(a[rows], "keys in order")
+    ref.check(b[rows], "keys permuted")
 
 
 def test_gemm_full_size_linearity_and_sampled_rows():
