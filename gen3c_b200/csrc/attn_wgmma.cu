@@ -16,16 +16,25 @@
 //                   ring and a V ring with their own full / empty barriers: step j of a consumer reads K_j and V_{j-1})
 //   warpgroups 1-2  consumers, 64 query rows each, software-pipelined with one S tile of lookahead:
 //                     prologue  S_0 = Q K_0^T, softmax, pack P_0
-//                     step j    [turn] issue S_j = Q K_j^T and O += P_{j-1} V_{j-1} [pass turn]; wait<1> (S_j done,
-//                               release K_j); row max and 2^(s - m) of S_j in place (m moves lazily, softmax_tile);
-//                               wait<0> (P.V done, release V_{j-1}); rescale O if m moved; pack P_j (bf16 A fragments
-//                               of the next P.V, from registers)
+//                     step j    [turn] issue S_j = Q K_j^T and O += P_{j-1} V_{j-1} [pass turn]; wait<1> (S_j done);
+//                               2^(s - m) of S_j in place against the current m, no row max (exp_tile); warpgroup
+//                               vote on the sum guard; in the rare case it fails, S_j again from K_j, wait<0> and the
+//                               exact softmax_tile (row max, m moves); release K_j; wait<0> (P.V done, release
+//                               V_{j-1}); rescale O if m moved; pack P_j (bf16 A fragments of the next P.V, from
+//                               registers)
 //                     epilogue  [turn] O += P_{n-1} V_{n-1} [pass turn]; wait<0>; normalise and store
 //                   so the softmax of step j runs under this warpgroup's own P.V(j-1).  Between the two warpgroups a turn
 //                   token (two mbarriers) alternates the MMA issue, so one warpgroup's softmax sits under the other's
 //                   MMAs instead of both drifting into the softmax together.  Both warpgroups take n_kv + 1 turns,
-//                   including one whose rows are all past Lq (it masks at the store).
-// The protocol (rings, wgmma group waits, turn token) is modelled in tests/test_attn_pingpong_model_cpu.py.
+//                   including one whose rows are all past Lq (it masks at the store).  The fallback's second S wgmma is
+//                   issued outside the turn: it only costs overlap, no barrier waits on it.
+// K_j is released after the guard decision (after the fallback's S on that path), not right after wait<1>: the fallback
+// reads K_j again.  That does not delay the producer: its next load into K_j's stage comes after its load of
+// V_{j+ATT_STAGES-1}, which waits for both consumers' release of V_{j-1}, and each consumer releases V_{j-1} after the
+// softmax of step j, with or without the guard.  The same order is why the fallback's read of K_j could not be overwritten
+// even by an early release; the release still comes after it, as the barrier's contract says.
+// The protocol (rings, wgmma group waits, turn token) is modelled in tests/test_attn_pingpong_model_cpu.py, with the sum
+// guard's fallback and K release in tests/test_attn_sum_guard_cpu.py.
 #include <cmath>
 #include <cstdlib>
 
@@ -48,6 +57,17 @@ static_assert(ATT_STAGES == 2, "attention: the consumer loop is unrolled for a r
 // Lazy rescale (softmax_tile): the reference row max moves only when a row's tile max exceeds it by more than this many
 // powers of two, so P <= 2^8 between moves.
 constexpr float ATT_RESCALE_LOG2 = 8.0f;
+// Sum guard of the steady-state tiles (exp_tile), G = 24: a tile exponentiated against the current reference is accepted
+// when each thread's partial row sums over its 32 columns stay below 2^G.  Every accepted P is then < 2^24, a row's tile
+// sum < 4 * 2^24 (four threads share a row) and l < n_kv * 2^26 (< 2^35 at the 440 tiles of Lk = 56 320; fp32 reaches
+// 2^128), and |O| <= l max|v| stays finite for max|v| < 2^128 / (n_kv 2^26), 2^93 at 440 tiles (2^104 with the lazy
+// rule alone).  A failing tile holds some P >= 2^G / 32 = 2^19, beyond ATT_RESCALE_LOG2, so its exact redo
+// (softmax_tile) moves m; that needs G >= 14.  G also bounds how far m trails the row max (< 24 instead of <= 8): the
+// fma argument of an exponential grows by that much, 2^-24 (|x - max x| + 24) of relative rounding, three orders of
+// magnitude below bf16 P's 2^-8; scaling P by a power of two leaves its bf16 rounding as it was, so only the fractional
+// part of m moves the roundings.  A fallback that moves m over a jump of more than 126 flushes earlier P of up to 2^G
+// (not 2^8) to 0 with alpha: each such key then held less than 2^-100 of its row's weight, all of them less than 2^-85.
+constexpr float ATT_GUARD = 16777216.0f;  // 2^G
 
 struct AttnParams {
   int Lq, Lk, heads;
@@ -81,6 +101,21 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return y;
 }
 
+// S <- P = 2^(S sl2 - m) in place against the reference m of this thread's two rows; acc[h] += this thread's sum of
+// its 32 P of row h.
+__device__ __forceinline__ void exp_tile(float (&s)[64], const float (&m_ref)[2], float (&acc)[2], float sl2) {
+  const float nm0 = -m_ref[0], nm1 = -m_ref[1];
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    s[4 * i] = ex2_approx(fmaf(s[4 * i], sl2, nm0));
+    s[4 * i + 1] = ex2_approx(fmaf(s[4 * i + 1], sl2, nm0));
+    s[4 * i + 2] = ex2_approx(fmaf(s[4 * i + 2], sl2, nm1));
+    s[4 * i + 3] = ex2_approx(fmaf(s[4 * i + 3], sl2, nm1));
+    acc[0] += s[4 * i] + s[4 * i + 1];
+    acc[1] += s[4 * i + 2] + s[4 * i + 3];
+  }
+}
+
 // Online softmax of one S tile (this thread's two rows), with a lazy reference.  The row max of the tile is exact; the
 // reference m the exponentials are taken against only moves when some row of the warp's 16 exceeds its m by more than
 // ATT_RESCALE_LOG2 (log2 units).  Then m <- max(m, row max), alpha = 2^(m_old - m_new), l <- l alpha, and the function
@@ -112,16 +147,7 @@ __device__ __forceinline__ bool softmax_tile(float (&s)[64], float (&m_ref)[2], 
       l_run[h] *= alpha[h];
     }
   }
-  const float nm0 = -m_ref[0], nm1 = -m_ref[1];
-#pragma unroll
-  for (int i = 0; i < 16; ++i) {
-    s[4 * i] = ex2_approx(fmaf(s[4 * i], sl2, nm0));
-    s[4 * i + 1] = ex2_approx(fmaf(s[4 * i + 1], sl2, nm0));
-    s[4 * i + 2] = ex2_approx(fmaf(s[4 * i + 2], sl2, nm1));
-    s[4 * i + 3] = ex2_approx(fmaf(s[4 * i + 3], sl2, nm1));
-    l_run[0] += s[4 * i] + s[4 * i + 1];
-    l_run[1] += s[4 * i + 2] + s[4 * i + 3];
-  }
+  exp_tile(s, m_ref, l_run, sl2);
   return !keep;
 }
 
@@ -159,7 +185,7 @@ __device__ __forceinline__ void issue_pv(float (&o)[64], const uint32_t (&pa)[32
 }
 
 // Last KV tile when Lk % 128 != 0: the TMA zero-filled the K rows past Lk, whose scores (0) would still enter the
-// softmax.  Columns >= `valid` (keys of this tile below Lk, 1..128) are set to -inf before the row max, so their
+// softmax.  Columns >= `valid` (keys of this tile below Lk, 1..128) are set to -inf before the softmax, so their
 // exponentials are 0.
 __device__ __forceinline__ void mask_key_tail(float (&s)[64], int valid, uint32_t lane) {
 #pragma unroll
@@ -346,11 +372,30 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
       ATT_TR(1 + c, 1);
       wgmma_wait<1>();  // S_j complete; P.V(j-1) may still run
       fence_regs(s);
-      if (tid == 0) mbar_arrive(&k_empty[kst]);
       ATT_TR(1 + c, 2);
       if (valid < ATT_TILE) mask_key_tail(s, valid, lane);
       // P_{j-1} (pa) and O are still read / written by the P.V in flight
-      const bool rescale = softmax_tile(s, m_ref, l_run, alpha, sl2);
+      // sum guard: this thread's partial row sums t against the current m, accepted when every thread of the
+      // warpgroup has both below ATT_GUARD (a NaN or inf fails the comparison); otherwise redone with softmax_tile
+      float t[2] = {0.f, 0.f};
+      exp_tile(s, m_ref, t, sl2);
+      const bool redo = bar_red_or(1 + c, 128, !(t[0] < ATT_GUARD && t[1] < ATT_GUARD));
+      if (redo) {  // warpgroup-uniform: S_j again from K_j, still held, then the exact softmax
+        wgmma_fence();
+        issue_s(s, dq, kst ? dk[1] : dk[0]);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(s);
+      }
+      if (tid == 0) mbar_arrive(&k_empty[kst]);
+      bool rescale = false;
+      if (redo) {
+        if (valid < ATT_TILE) mask_key_tail(s, valid, lane);
+        rescale = softmax_tile(s, m_ref, l_run, alpha, sl2);
+      } else {
+        l_run[0] += t[0];
+        l_run[1] += t[1];
+      }
       ATT_TR(1 + c, 3);
       wgmma_wait<0>();
       fence_regs(o);
@@ -379,7 +424,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
       ph ^= 1u;
     }
     if constexpr (kVTokenMajor) {
-      // ---- the last KV tile: the same step with the keys past Lk masked before the row max ----
+      // ---- the last KV tile: the same step with the keys past Lk masked before the softmax ----
       if (n_kv > 1) {
         j = n_kv - 1;
         step(j & 1, (j - 1) & 1, ((uint32_t)j >> 1) & 1u, ((uint32_t)(j - 1) >> 1) & 1u, p.Lk - j * ATT_TILE);

@@ -187,6 +187,22 @@ __device__ __forceinline__ void mbar_wait_ns_or_exit(uint64_t* bar, uint32_t par
   }
 }
 
+// OR of `pred` over the `nthreads` threads (a multiple of 32, every one of them executing this) that meet at named
+// barrier `id` (not 0, which __syncthreads uses): all of them get the same result, so a branch on it is uniform over
+// their warps, e.g. around a wgmma that all four warps of a warpgroup must issue together.
+__device__ __forceinline__ bool bar_red_or(uint32_t id, uint32_t nthreads, bool pred) {
+  uint32_t r;
+  asm volatile(
+      "{\n\t.reg .pred P, Q;\n\t"
+      "setp.ne.u32 P, %1, 0;\n\t"
+      "bar.red.or.pred Q, %2, %3, P;\n\t"
+      "selp.u32 %0, 1, 0, Q;\n\t}\n"
+      : "=r"(r)
+      : "r"((uint32_t)pred), "r"(id), "r"(nthreads)
+      : "memory");
+  return r != 0;
+}
+
 // ----------------------------------------------------------------------------------------------
 // TMA loads (tile mode, mbarrier completion)
 // ----------------------------------------------------------------------------------------------
