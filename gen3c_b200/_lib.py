@@ -118,6 +118,10 @@ SIGNATURES = {
     "g3c_dit_read_modulation": (_I, [_P, _F, _P, _P, _P]),
     "g3c_dit_read_step": (_I, [_P, _P, _P, _P, _P, _P]),
     "g3c_attn_fwd_gated": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _F, _P, C.c_uint32, _I, _P, _P]),
+    "g3c_dit_cp_region": (_I, [_P, C.POINTER(_P), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "g3c_dit_cp_attach": (_I, [_P, C.POINTER(_P), _I]),
+    "g3c_dit_cfg_region": (_I, [_P, C.POINTER(_P), C.POINTER(C.c_int64)]),
+    "g3c_dit_cfg_attach": (_I, [_P, _P]),
 }
 
 _lib = None

@@ -155,6 +155,8 @@ struct g3c_dit {
   size_t cp_region_bytes = 0, off_k[2] = {0, 0}, off_vt[2] = {0, 0}, off_flags = 0;
   void* peer_base[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   bool peers_open = false;
+  // peer_base holds device pointers of this process (g3c_dit_cp_attach), not IPC mappings: never close them
+  bool peers_attached = false;
   uint32_t kv_seq = 0;
   // pinned ring of sequence numbers: the copy engine writes flags[rank] = seq on every peer by copying 4 bytes from
   // here after the K / V^T copies (no kernel on the side stream: a flag kernel queued behind a grid whose CTAs spin
@@ -185,6 +187,7 @@ struct g3c_dit {
   int cfg_role = -1;
   void* cfg_region = nullptr;
   void* cfg_peer = nullptr;
+  bool cfg_attached = false;  // cfg_peer is a device pointer of this process (g3c_dit_cfg_attach), not an IPC mapping
   size_t cfg_slot_bytes = 0;
   uint32_t cfg_seq = 0;
   // attention kernel: ns spent polling peer flags (summed over CTAs), CTA count of those launches
@@ -624,15 +627,18 @@ static void free_cp_region(g3c_dit* h) {
   // before unmapping.  The cross-rank half of the hazard (peers still pushing into OUR region) is closed by the caller's
   // barrier on the cp group (gen3c_b200/dit.py::_teardown_barrier).
   if (h->cp_region || h->cfg_region) cudaDeviceSynchronize();
-  if (h->cfg_peer) cudaIpcCloseMemHandle(h->cfg_peer);
+  if (h->cfg_peer && !h->cfg_attached) cudaIpcCloseMemHandle(h->cfg_peer);
   h->cfg_peer = nullptr;
+  h->cfg_attached = false;
   if (h->cfg_region) cudaFree(h->cfg_region);
   h->cfg_region = nullptr;
   for (int r = 0; r < 8; ++r) {
-    if (h->peer_base[r] && h->peer_base[r] != h->cp_region) cudaIpcCloseMemHandle(h->peer_base[r]);
+    if (h->peer_base[r] && h->peer_base[r] != h->cp_region && !h->peers_attached)
+      cudaIpcCloseMemHandle(h->peer_base[r]);
     h->peer_base[r] = nullptr;
   }
   h->peers_open = false;
+  h->peers_attached = false;
   if (h->cp_region) cudaFree(h->cp_region);
   h->cp_region = nullptr;
   h->cp_region_bytes = 0;
@@ -1063,6 +1069,67 @@ int g3c_dit_read_step(g3c_dit_t* h, void* xtilde, void* xin, void* oc, void* ou,
   G3C_CUDA(cudaMemcpyAsync(xin, h->lat_xin, bytes, cudaMemcpyDeviceToDevice, st));
   G3C_CUDA(cudaMemcpyAsync(oc, h->step_oc, bytes, cudaMemcpyDeviceToDevice, st));
   G3C_CUDA(cudaMemcpyAsync(ou, h->step_ou, bytes, cudaMemcpyDeviceToDevice, st));
+  return G3C_OK;
+}
+
+int g3c_dit_cp_region(g3c_dit_t* h, void** base, int64_t* off_k2, int64_t* off_vt2, int64_t* off_flags) {
+  G3C_REQUIRE(h && base && off_k2 && off_vt2 && off_flags, "dit_cp_region: null argument");
+  if (!h->cp_region) {
+    set_error("dit_cp_region: no context-parallel region (enable_cp without NCCL id, then set_shape)");
+    return G3C_ESTATE;
+  }
+  *base = h->cp_region;
+  for (int s = 0; s < 2; ++s) {
+    off_k2[s] = (int64_t)h->off_k[s];
+    off_vt2[s] = (int64_t)h->off_vt[s];
+  }
+  *off_flags = (int64_t)h->off_flags;
+  return G3C_OK;
+}
+
+int g3c_dit_cp_attach(g3c_dit_t* h, const void* const* bases, int n) {
+  G3C_REQUIRE(h && bases, "dit_cp_attach: null argument");
+  if (!h->cp_region) {
+    set_error("dit_cp_attach: no context-parallel region (enable_cp without NCCL id, then set_shape)");
+    return G3C_ESTATE;
+  }
+  if (h->peers_open && !h->peers_attached) {
+    set_error("dit_cp_attach: the peers' regions are already imported (g3c_dit_cp_import)");
+    return G3C_ESTATE;
+  }
+  G3C_REQUIRE(n == h->cp_size, "dit_cp_attach: need one region per rank (%d), got %d", h->cp_size, n);
+  for (int r = 0; r < n; ++r) G3C_REQUIRE(bases[r], "dit_cp_attach: null region of rank %d", r);
+  G3C_REQUIRE(bases[h->cp_rank] == h->cp_region, "dit_cp_attach: entry %d must be this handle's own region",
+              h->cp_rank);
+  for (int r = 0; r < n; ++r) h->peer_base[r] = const_cast<void*>(bases[r]);
+  h->peers_attached = true;
+  h->peers_open = true;
+  return G3C_OK;
+}
+
+int g3c_dit_cfg_region(g3c_dit_t* h, void** base, int64_t* slot_bytes) {
+  G3C_REQUIRE(h && base && slot_bytes, "dit_cfg_region: null argument");
+  if (!h->cfg_region) {
+    set_error("dit_cfg_region: no exchange region (enable_cfg_parallel, then set_shape)");
+    return G3C_ESTATE;
+  }
+  *base = h->cfg_region;
+  *slot_bytes = (int64_t)h->cfg_slot_bytes;
+  return G3C_OK;
+}
+
+int g3c_dit_cfg_attach(g3c_dit_t* h, const void* partner_base) {
+  G3C_REQUIRE(h && partner_base, "dit_cfg_attach: null argument");
+  if (!h->cfg_region) {
+    set_error("dit_cfg_attach: no exchange region (enable_cfg_parallel, then set_shape)");
+    return G3C_ESTATE;
+  }
+  if (h->cfg_peer && !h->cfg_attached) {
+    set_error("dit_cfg_attach: the partner's region is already imported (g3c_dit_cfg_import)");
+    return G3C_ESTATE;
+  }
+  h->cfg_peer = const_cast<void*>(partner_base);
+  h->cfg_attached = true;
   return G3C_OK;
 }
 

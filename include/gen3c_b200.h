@@ -343,6 +343,23 @@ int g3c_dit_read_step(g3c_dit_t* h, void* xtilde, void* xin, void* oc, void* ou,
 int g3c_attn_fwd_gated(const void* q, const void* k, const void* vt, void* o, int Lq, int Lk, int heads,
                        int ldq, int ldk, int ldo, int vt_chunk_len, float scale,
                        const uint32_t* flags, uint32_t seq, int first, unsigned long long* wait_ns, void* stream);
+/* The two peer-memory exchanges of the engine wired inside one process, so that every rank's handle can run on one
+ * device, one after another.  g3c_dit_cp_region: this rank's context-parallel region (peer-memory mode, after
+ * g3c_dit_set_shape) and its layout, as byte offsets from base: K of layer-parity set s (set = seq & 1 of the
+ * self-attention layer) bf16 [cp][L][D] at off_k2[s], V^T bf16 [cp][D][L] at off_vt2[s], and uint32 arrival flags
+ * [2][8] at off_flags (flags[s*8 + r] = seq of the last layer whose rank-r chunk landed in set s).  G3C_ESTATE without
+ * such a region.  g3c_dit_cp_attach: g3c_dit_cp_import with the device pointers of the n = cp_size regions (from
+ * g3c_dit_cp_region of each rank's handle, in rank order; entry cp_rank must be this handle's own region) instead of IPC
+ * handles; G3C_ESTATE without a region or after g3c_dit_cp_import, G3C_EINVAL for a wrong n or entry.  Attached
+ * pointers are never unmapped by this handle; the regions belong to their own handles, so every handle must be
+ * synchronised before another one's region is freed. */
+int g3c_dit_cp_region(g3c_dit_t* h, void** base, int64_t* off_k2, int64_t* off_vt2, int64_t* off_flags);
+int g3c_dit_cp_attach(g3c_dit_t* h, const void* const* bases, int n);
+/* The same for CFG parallelism: this rank's exchange region (2 slots of slot_bytes, the partner's output of step seq in
+ * slot seq & 1, then uint32 flags [2] = seq of the output in each slot) and g3c_dit_cfg_import with the partner's region
+ * pointer.  G3C_ESTATE without an exchange region (enable_cfg_parallel, then set_shape) or after g3c_dit_cfg_import. */
+int g3c_dit_cfg_region(g3c_dit_t* h, void** base, int64_t* slot_bytes);
+int g3c_dit_cfg_attach(g3c_dit_t* h, const void* partner_base);
 
 #ifdef __cplusplus
 }
