@@ -203,6 +203,11 @@ __device__ __forceinline__ bool bar_red_or(uint32_t id, uint32_t nthreads, bool 
   return r != 0;
 }
 
+// Named barrier `id` (not 0, which __syncthreads uses) over `nthreads` threads (a multiple of 32).
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(nthreads) : "memory");
+}
+
 // ----------------------------------------------------------------------------------------------
 // TMA loads (tile mode, mbarrier completion)
 // ----------------------------------------------------------------------------------------------

@@ -9,8 +9,10 @@
 // Structure (one persistent CTA per SM, 384 threads = three warpgroups):
 //   warpgroup 0   TMA producer : one thread, cp.async.bulk.tensor A/B tiles -> smem ring (kStages), mbarrier tx
 //   warpgroups 1-2 consumers   : wgmma 64 x BN x 16 each (rows 0-63 / 64-127 of the 128-row tile), accumulators in
-//                                registers, fused epilogue straight from the registers to global memory
-// The producer runs ahead into the next tile while the consumers run the epilogue of the current one.
+//                                registers, fused epilogue from the registers into a shared-memory staging buffer
+//                                that TMA stores to global memory (or, for the gated residual, reduce-adds into it)
+// The producer runs ahead into the next tile while the consumers run the epilogue of the current one, and the last
+// TMA store of a tile drains while the consumers already run the next tile's MMAs.
 //
 // FP8 (e4m3) instantiation (kFp8): the operands are row-quantized codes, D[m,n] = (sum_k A8[m,k] B8[n,k]) *
 // scale_a[m] * scale_b[n].  A k-block is then 128 codes instead of 64 bf16: still 128 bytes, one swizzle span, so the
@@ -33,6 +35,8 @@ constexpr int GEMM_THREADS = 384;
 struct GemmParams {
   int M, N, K;
   int ldd;             // leading dimension of D in elements
+  int n_tma;           // columns [0, n_tma) leave through the TMA map of D: N rounded down to 16 bytes (TMA writes
+                       // whole 16-byte pieces of a row); the rest of the row is stored by the threads
   void* D;             // bf16 or f32
   const float* gate;   // [N] for EPI_GATED_RESIDUAL
   int num_m_blk, num_n_blk, num_k_blk;
@@ -51,14 +55,22 @@ struct GemmParams {
 // the rotate-half RoPE, applied to the fp32 accumulators of one head while they are still in registers.
 constexpr int EPI_NORM_ROPE_BF16 = 4;
 
+// Output boxes: 64 rows (one consumer warpgroup) x 128 bytes (64 bf16 / 32 f32 columns, one swizzle span).
+constexpr int OUT_BOX_ROWS = 64;
+constexpr int OUT_BOX_BYTES = OUT_BOX_ROWS * 128;
+
 template <int BN>
 struct GemmSmem {
   static constexpr int kABytes = BM * BK * 2;
   static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kStages = (192 * 1024) / kStageBytes;  // 4 / 6 / 8 stages for BN = 256 / 128 / 64
+  static constexpr int kRingBytes = kStages * kStageBytes;
+  static constexpr int kStagingBytes = 2 * OUT_BOX_BYTES;      // per consumer warpgroup: two output boxes per round
   static constexpr int kBarBytes = 256;
-  static constexpr int kTotal = kStages * kStageBytes + kBarBytes + 1024;  // + alignment slack
+  static constexpr int kTotal = kRingBytes + 2 * kStagingBytes + kBarBytes + 1024;  // + alignment slack
+  static_assert(kRingBytes % 1024 == 0, "the staging buffers need the 1024-byte alignment of the 128-byte swizzle");
+  static_assert(kTotal <= 227 * 1024, "shared memory per CTA");
 };
 
 __device__ __forceinline__ float gelu_erf(float x) {
@@ -78,6 +90,96 @@ __device__ __forceinline__ void tile_coords(const GemmParams& p, int tile, int& 
   n_blk = n0 + rem - m_blk * width;
 }
 
+// Output staging of one consumer warpgroup.  Its 64 rows of a tile leave in rounds of at most two output boxes: the
+// warpgroup writes a round into its staging half in the layout of the TMA box with the 128-byte swizzle (16-byte chunk
+// j of box row r at chunk j ^ (r % 8)), and one thread stores the boxes to D, or for the gated residual reduce-adds them
+// into x in L2 (every element of x still has exactly one owning tile, so the sum stays deterministic).  TMA clips rows
+// >= M and columns >= n_tma.  A round only waits until the previous round's boxes have been read out of shared memory, so
+// the last round of a tile drains while the warpgroup already runs the next tile's MMAs.
+struct OutStage {
+  uint8_t* base;    // this warpgroup's staging half (1024-byte aligned)
+  uint32_t buf;     // its shared-window address
+  uint32_t bar_id;  // named barrier of the warpgroup's 128 threads
+  bool leader;      // the one thread that issues, commits and waits for the TMA stores
+  uint32_t row;     // byte offset of the thread's first accumulator row r = 16 warp + lane / 4 inside a box
+  uint32_t sw;      // lane / 4 = r % 8, the same for both of the thread's rows (r, r + 8): the swizzle of its chunks
+  uint32_t col_q;   // 2 (lane % 4): the thread's first column inside an 8-column accumulator group
+};
+
+// The thread's staging addresses for elements of kEsize bytes: `thr` is its first value pair in row r of box 0 before
+// the swizzle, `sw16` = (r % 8) << 4 the XOR on the chunk bits [4, 7) of a box row.  Both are produced after the
+// mainloop (an empty asm the compiler cannot look through), so that the addresses are not hoisted into it and kept
+// live beside the accumulators.
+struct StageAddr {
+  uint32_t thr, sw16;
+};
+template <int kEsize>
+__device__ __forceinline__ StageAddr stage_addr_base(const OutStage& o) {
+  StageAddr a{o.buf + o.row + o.col_q * kEsize, o.sw << 4};
+  asm volatile("" : "+r"(a.thr), "+r"(a.sw16));
+  return a;
+}
+// Shared address of the thread's value pair for accumulator group i (columns 8i + col_q + {0, 1} of the tile; only
+// i modulo the groups of one round matters) and row half h (rows r + 8h).  The chunk bits of `thr` + the column byte
+// offset are those of the unswizzled row (the buffer is 1024-byte aligned and rows are 128 bytes), so the swizzle is
+// one XOR.
+template <int kEsize>
+__device__ __forceinline__ uint32_t stage_addr(const StageAddr& a, int i, int h) {
+  constexpr int kGroupsPerBox = 128 / (8 * kEsize);  // 8 (bf16) or 4 (f32)
+  const uint32_t col_byte = (uint32_t)(i % kGroupsPerBox) * 8 * kEsize;
+  const uint32_t box = (uint32_t)(i / kGroupsPerBox) % 2;
+  return ((a.thr + h * 8 * 128 + col_byte) ^ a.sw16) + box * OUT_BOX_BYTES;
+}
+__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;\n" ::"r"(addr), "r"(v));
+}
+__device__ __forceinline__ void st_shared_f32x2(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};\n" ::"r"(addr), "f"(a), "f"(b));
+}
+// Before the warpgroup writes a round: the previous round's boxes have been read out of the staging half.
+__device__ __forceinline__ void stage_acquire(const OutStage& o) {
+  if (o.leader) tma_store_wait_read<0>();
+  named_bar_sync(o.bar_id, 128);
+}
+// After it: make the writes visible to the async proxy, then one thread stores `nbox` boxes (columns col0 + b * 128
+// bytes, rows row0 ..) and commits them as one bulk group.  Columns [n_tma, N) (less than 16 bytes of a row, only when
+// N is not a multiple of 16 bytes) are copied from the staging buffer by the warpgroup's threads.
+template <bool kReduce, int kEsize>
+__device__ __forceinline__ void stage_issue(const OutStage& o, const CUtensorMap* tmD, int nbox, int box_cols, int col0,
+                                            int row0, const GemmParams& p) {
+  fence_proxy_async();
+  named_bar_sync(o.bar_id, 128);
+  if (p.n_tma < p.N && p.n_tma >= col0 && p.n_tma < col0 + nbox * box_cols) {
+    const int ntail = p.N - p.n_tma, tid = (int)(threadIdx.x % 128);
+#pragma unroll 1
+    for (int e = tid; e < OUT_BOX_ROWS * ntail; e += 128) {
+      const int r = e / ntail, col = p.n_tma + e % ntail;
+      if (row0 + r >= p.M) break;
+      const uint32_t byte = (uint32_t)((col - col0) % box_cols) * kEsize;
+      const uint32_t off = (uint32_t)((col - col0) / box_cols) * OUT_BOX_BYTES + r * 128 +
+                           ((((byte >> 4) ^ (uint32_t)(r % 8))) << 4) + (byte & 15);
+      const size_t g = (size_t)(row0 + r) * p.ldd + col;
+      uint32_t v;
+      if constexpr (kEsize == 2) {
+        asm volatile("ld.shared.u16 %0, [%1];\n" : "=r"(v) : "r"(o.buf + off));
+        reinterpret_cast<uint16_t*>(p.D)[g] = (uint16_t)v;
+      } else {
+        asm volatile("ld.shared.b32 %0, [%1];\n" : "=r"(v) : "r"(o.buf + off));
+        float* d = reinterpret_cast<float*>(p.D) + g;
+        *d = kReduce ? *d + __uint_as_float(v) : __uint_as_float(v);  // RN(x + RN(gate * acc)), as the TMA reduction
+      }
+    }
+  }
+  if (o.leader && row0 < p.M) {
+    for (int b = 0; b < nbox; ++b) {
+      if (col0 + b * box_cols >= p.n_tma) break;
+      if constexpr (kReduce) tma_reduce_add_2d(tmD, o.base + b * OUT_BOX_BYTES, col0 + b * box_cols, row0);
+      else tma_store_2d(tmD, o.base + b * OUT_BOX_BYTES, col0 + b * box_cols, row0);
+    }
+    tma_store_commit();
+  }
+}
+
 // Accumulator layout of wgmma m64nNk16 (f32): thread t of the warpgroup holds, for i in [0, N/8),
 //   acc[4i + 0], acc[4i + 1] -> row 16 * (t / 32) + (t % 32) / 4,     columns 8i + 2 (t % 4) + {0, 1}
 //   acc[4i + 2], acc[4i + 3] -> the same columns eight rows further down.
@@ -85,9 +187,14 @@ __device__ __forceinline__ void tile_coords(const GemmParams& p, int tile, int& 
 // are spread over the four threads of a quad (reduced with two shuffles), and the rotate-half partners c and c + 64
 // (accumulator indices i and i + 8) sit in the same thread.  reference: module/attention.py:263-266 (to_q/to_k =
 // Linear + RMSNorm) and :268-283 (apply_rotary_pos_emb); same arithmetic as k_rmsnorm_rope (dit_elementwise.cu).
+// One head is one round of two bf16 boxes (columns c and c + 64).
 template <int BN>
-__device__ __forceinline__ void epilogue_norm_rope(const float (&acc)[BN / 2], const GemmParams& p, int row_a, int col_q,
+__device__ __forceinline__ void epilogue_norm_rope(const float (&acc)[BN / 2], const GemmParams& p,
+                                                   const CUtensorMap* tmD, const OutStage& o, int row_a, int row0,
                                                    int n_base) {
+  const float* __restrict__ gamma = p.nr_gamma;
+  const float* __restrict__ cs_tab = p.nr_cs;
+  const int col_q = (int)o.col_q;
 #pragma unroll
   for (int hd = 0; hd < BN / 128; ++hd) {
     if (n_base + hd * 128 >= p.N) break;
@@ -102,24 +209,25 @@ __device__ __forceinline__ void epilogue_norm_rope(const float (&acc)[BN / 2], c
       ss[h] += __shfl_xor_sync(0xffffffffu, ss[h], 1);
       ss[h] += __shfl_xor_sync(0xffffffffu, ss[h], 2);
     }
+    stage_acquire(o);
+    const StageAddr sa = stage_addr_base<2>(o);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int row = row_a + 8 * h;
       if (row >= p.M) continue;
       const float rstd = rsqrtf(ss[h] * (1.0f / 128.0f) + p.nr_eps);
-      const float* cs = p.nr_cs ? p.nr_cs + (size_t)row * 128 : nullptr;
-      __nv_bfloat16* dptr = reinterpret_cast<__nv_bfloat16*>(p.D) + (size_t)row * p.ldd + n_base + hd * 128;
+      const float* cs = cs_tab ? cs_tab + (size_t)row * 128 : nullptr;
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         const int c = 8 * i + col_q;  // column inside the head, < 64; the partner is c + 64
-        const float2 ga = *reinterpret_cast<const float2*>(p.nr_gamma + c);
-        const float2 gb = *reinterpret_cast<const float2*>(p.nr_gamma + 64 + c);
+        const float2 ga = __ldg(reinterpret_cast<const float2*>(gamma + c));
+        const float2 gb = __ldg(reinterpret_cast<const float2*>(gamma + 64 + c));
         const int ia = 4 * (16 * hd + i) + 2 * h, ib = 4 * (16 * hd + i + 8) + 2 * h;
         float a[2] = {acc[ia] * (rstd * ga.x), acc[ia + 1] * (rstd * ga.y)};
         float b[2] = {acc[ib] * (rstd * gb.x), acc[ib + 1] * (rstd * gb.y)};
         if (cs) {
-          const float2 co = *reinterpret_cast<const float2*>(cs + c);
-          const float2 si = *reinterpret_cast<const float2*>(cs + 64 + c);
+          const float2 co = __ldg(reinterpret_cast<const float2*>(cs + c));
+          const float2 si = __ldg(reinterpret_cast<const float2*>(cs + 64 + c));
           const float cv[2] = {co.x, co.y}, sv[2] = {si.x, si.y};
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
@@ -128,27 +236,30 @@ __device__ __forceinline__ void epilogue_norm_rope(const float (&acc)[BN / 2], c
             b[e] = m;
           }
         }
-        *reinterpret_cast<uint32_t*>(dptr + c) = pack_bf16x2(a[0], a[1]);
-        *reinterpret_cast<uint32_t*>(dptr + 64 + c) = pack_bf16x2(b[0], b[1]);
+        st_shared_b32(stage_addr<2>(sa, i, h), pack_bf16x2(a[0], a[1]));
+        st_shared_b32(stage_addr<2>(sa, i + 8, h), pack_bf16x2(b[0], b[1]));
       }
     }
+    stage_issue<false, 2>(o, tmD, 2, 64, n_base + hd * 128, row0, p);
   }
 }
 
 // fp8: dequantise the accumulators in place, acc * scale_a[row] * scale_b[col], before any epilogue arithmetic (the
-// RMSNorm of the fused to_q / to_k epilogue must see the dequantised values).  Rows / columns past M / N keep their
-// zero accumulators (scale 0): the epilogue does not store them.
+// RMSNorm of the fused to_q / to_k epilogue must see the dequantised values).  Rows / columns past M / N get zero
+// accumulators (scale 0): TMA does not store them.
 template <int BN>
 __device__ __forceinline__ void dequantise(float (&acc)[BN / 2], const GemmParams& p, int row_a, int col_q, int n_base) {
+  const float* __restrict__ scale_a = p.scale_a;
+  const float* __restrict__ scale_b = p.scale_b;
   float sa[2];
 #pragma unroll
-  for (int h = 0; h < 2; ++h) sa[h] = row_a + 8 * h < p.M ? p.scale_a[row_a + 8 * h] : 0.f;
+  for (int h = 0; h < 2; ++h) sa[h] = row_a + 8 * h < p.M ? __ldg(scale_a + row_a + 8 * h) : 0.f;
 #pragma unroll
   for (int i = 0; i < BN / 8; ++i) {
     const int col = n_base + 8 * i + col_q;
     float2 sb = make_float2(0.f, 0.f);
-    if (col + 1 < p.N) sb = *reinterpret_cast<const float2*>(p.scale_b + col);
-    else if (col < p.N) sb.x = p.scale_b[col];
+    if (col + 1 < p.N) sb = __ldg(reinterpret_cast<const float2*>(scale_b + col));
+    else if (col < p.N) sb.x = __ldg(scale_b + col);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       acc[4 * i + 2 * h] = acc[4 * i + 2 * h] * sa[h] * sb.x;
@@ -157,56 +268,58 @@ __device__ __forceinline__ void dequantise(float (&acc)[BN / 2], const GemmParam
   }
 }
 
+// bf16 / GELU / f32 outputs, and the gated residual: x += RN(gate * acc), reduce-added by TMA.  A round is two boxes
+// (128 bf16 or 64 f32 columns) or the whole tile when it is narrower.
 template <int BN, int EPI>
-__device__ __forceinline__ void epilogue(const float (&acc)[BN / 2], const GemmParams& p, int row_a, int col_q,
-                                         int n_base) {
-  if constexpr (EPI == EPI_NORM_ROPE_BF16) {
-    epilogue_norm_rope<BN>(acc, p, row_a, col_q, n_base);
-  } else {
+__device__ __forceinline__ void epilogue(const float (&acc)[BN / 2], const GemmParams& p, const CUtensorMap* tmD,
+                                         const OutStage& o, int row0, int n_base) {
+  constexpr bool kGated = EPI == G3C_EPI_GATED_RESIDUAL_F32;
+  constexpr int kEsize = (kGated || EPI == G3C_EPI_F32) ? 4 : 2;
+  constexpr int kBoxCols = 128 / kEsize;
+  constexpr int kRoundGroups = 2 * kBoxCols / 8 < BN / 8 ? 2 * kBoxCols / 8 : BN / 8;
+  constexpr int kRoundBoxes = (8 * kRoundGroups + kBoxCols - 1) / kBoxCols;
+  const float* __restrict__ gate = p.gate;
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = row_a + 8 * h;
-      if (row >= p.M) continue;
+  for (int rd = 0; rd < BN / 8 / kRoundGroups; ++rd) {
+    float2 g[kGated ? kRoundGroups : 1];
+    if constexpr (kGated) {
+      // the round's gate pairs, loaded ahead of the staging wait and the arithmetic
 #pragma unroll
-      for (int i = 0; i < BN / 8; ++i) {
-        const int col = n_base + 8 * i + col_q;
-        if (col >= p.N) continue;
-        const bool pair = col + 1 < p.N;
-        float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
-        if constexpr (EPI == G3C_EPI_BF16 || EPI == G3C_EPI_GELU_BF16) {
-          if constexpr (EPI == G3C_EPI_GELU_BF16) {
-            v0 = gelu_erf(v0);
-            v1 = gelu_erf(v1);
-          }
-          __nv_bfloat16* dptr = reinterpret_cast<__nv_bfloat16*>(p.D) + (size_t)row * p.ldd + col;
-          if (pair) *reinterpret_cast<uint32_t*>(dptr) = pack_bf16x2(v0, v1);
-          else dptr[0] = __float2bfloat16_rn(v0);
-        } else {
-          float* dptr = reinterpret_cast<float*>(p.D) + (size_t)row * p.ldd + col;
-          if constexpr (EPI == G3C_EPI_GATED_RESIDUAL_F32) {
-            // x += gate * acc on the fp32 residual stream; every element has exactly one owner
-            if (pair) {
-              const float2 g = *reinterpret_cast<const float2*>(p.gate + col);
-              float2 x = *reinterpret_cast<float2*>(dptr);
-              x.x = fmaf(g.x, v0, x.x);
-              x.y = fmaf(g.y, v1, x.y);
-              *reinterpret_cast<float2*>(dptr) = x;
-            } else {
-              dptr[0] = fmaf(p.gate[col], v0, dptr[0]);
-            }
-          } else {
-            if (pair) *reinterpret_cast<float2*>(dptr) = make_float2(v0, v1);
-            else dptr[0] = v0;
-          }
-        }
+      for (int j = 0; j < kRoundGroups; ++j) {
+        const int col = n_base + 8 * (rd * kRoundGroups + j) + (int)o.col_q;
+        g[j] = make_float2(0.f, 0.f);
+        if (col + 1 < p.N) g[j] = __ldg(reinterpret_cast<const float2*>(gate + col));
+        else if (col < p.N) g[j].x = __ldg(gate + col);
       }
     }
+    stage_acquire(o);
+    const StageAddr sa = stage_addr_base<kEsize>(o);
+#pragma unroll
+    for (int j = 0; j < kRoundGroups; ++j) {
+      const int i = rd * kRoundGroups + j;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
+        if constexpr (EPI == G3C_EPI_GELU_BF16) {
+          v0 = gelu_erf(v0);
+          v1 = gelu_erf(v1);
+        }
+        if constexpr (kGated) {
+          v0 = g[j].x * v0;
+          v1 = g[j].y * v1;
+        }
+        if constexpr (kEsize == 2) st_shared_b32(stage_addr<2>(sa, i, h), pack_bf16x2(v0, v1));
+        else st_shared_f32x2(stage_addr<4>(sa, i, h), v0, v1);
+      }
+    }
+    stage_issue<kGated, kEsize>(o, tmD, kRoundBoxes, kBoxCols, n_base + rd * 8 * kRoundGroups, row0, p);
   }
 }
 
 template <int BN, int EPI, bool kFp8>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-    k_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+    k_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+           const __grid_constant__ CUtensorMap tmD, const GemmParams p) {
   using S = GemmSmem<BN>;
   constexpr int kStages = S::kStages;
   extern __shared__ uint8_t smem_raw[];
@@ -214,7 +327,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + kStages * S::kABytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * S::kStageBytes);
+  uint8_t* staging = smem + S::kRingBytes;  // [2][kStagingBytes], one half per consumer warpgroup
+  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + 2 * S::kStagingBytes);
   uint64_t* full = bars;              // [kStages]
   uint64_t* empty = bars + kStages;   // [kStages]
 
@@ -224,6 +338,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    tma_prefetch_desc(&tmD);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full[i], 1);
       mbar_init(&empty[i], 2);  // one arrive per consumer warpgroup
@@ -259,6 +374,14 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     setmaxnreg_inc<232>();
     const uint32_t c = wg - 1;
     const uint32_t warp = tid / 32, lane = tid % 32;
+    OutStage out;
+    out.base = staging + c * S::kStagingBytes;
+    out.buf = smem_u32(out.base);
+    out.bar_id = 1 + c;
+    out.leader = tid == 0;
+    out.row = (16 * warp + lane / 4) * 128;
+    out.sw = lane / 4;
+    out.col_q = 2 * (lane % 4);
     uint32_t stage = 0, phase = 0;
     float acc[BN / 2];
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -325,15 +448,19 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         fence_regs(acc);
         if (tid == 0) mbar_arrive(&empty[prev_stage]);
       }
-      const int row_a = m_blk * BM + (int)(c * 64 + warp * 16 + lane / 4), col_q = (int)(2 * (lane % 4));
-      if constexpr (kFp8) dequantise<BN>(acc, p, row_a, col_q, n_blk * BN);
-      epilogue<BN, EPI>(acc, p, row_a, col_q, n_blk * BN);
+      const int row0 = m_blk * BM + (int)c * 64, row_a = row0 + (int)(warp * 16 + lane / 4);
+      if constexpr (kFp8) dequantise<BN>(acc, p, row_a, (int)out.col_q, n_blk * BN);
+      if constexpr (EPI == EPI_NORM_ROPE_BF16) epilogue_norm_rope<BN>(acc, p, &tmD, out, row_a, row0, n_blk * BN);
+      else epilogue<BN, EPI>(acc, p, &tmD, out, row0, n_blk * BN);
     }
+    // the staging buffer must outlive the reads of the last boxes, and the stores complete before the CTA retires
+    if (out.leader) tma_store_wait_all<0>();
   }
 }
 
 template <int BN, int EPI, bool kFp8>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t st) {
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD, const GemmParams& p,
+                       cudaStream_t st) {
   using S = GemmSmem<BN>;
   static bool configured = false;
   if (!configured) {
@@ -342,20 +469,21 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Gem
   }
   int tiles = p.num_m_blk * p.num_n_blk;
   int grid = tiles < sm_count() ? tiles : sm_count();
-  k_gemm<BN, EPI, kFp8><<<grid, GEMM_THREADS, S::kTotal, st>>>(tmA, tmB, p);
+  k_gemm<BN, EPI, kFp8><<<grid, GEMM_THREADS, S::kTotal, st>>>(tmA, tmB, tmD, p);
   G3C_CUDA(cudaGetLastError());
   return G3C_OK;
 }
 
 template <int BN, bool kFp8>
-static int dispatch_epi(int epi, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t st) {
+static int dispatch_epi(int epi, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD,
+                        const GemmParams& p, cudaStream_t st) {
   switch (epi) {
-    case G3C_EPI_BF16: return launch_gemm<BN, G3C_EPI_BF16, kFp8>(tmA, tmB, p, st);
-    case G3C_EPI_GELU_BF16: return launch_gemm<BN, G3C_EPI_GELU_BF16, kFp8>(tmA, tmB, p, st);
-    case G3C_EPI_GATED_RESIDUAL_F32: return launch_gemm<BN, G3C_EPI_GATED_RESIDUAL_F32, kFp8>(tmA, tmB, p, st);
-    case G3C_EPI_F32: return launch_gemm<BN, G3C_EPI_F32, kFp8>(tmA, tmB, p, st);
+    case G3C_EPI_BF16: return launch_gemm<BN, G3C_EPI_BF16, kFp8>(tmA, tmB, tmD, p, st);
+    case G3C_EPI_GELU_BF16: return launch_gemm<BN, G3C_EPI_GELU_BF16, kFp8>(tmA, tmB, tmD, p, st);
+    case G3C_EPI_GATED_RESIDUAL_F32: return launch_gemm<BN, G3C_EPI_GATED_RESIDUAL_F32, kFp8>(tmA, tmB, tmD, p, st);
+    case G3C_EPI_F32: return launch_gemm<BN, G3C_EPI_F32, kFp8>(tmA, tmB, tmD, p, st);
     case EPI_NORM_ROPE_BF16:
-      if constexpr (BN >= 128) return launch_gemm<BN, EPI_NORM_ROPE_BF16, kFp8>(tmA, tmB, p, st);
+      if constexpr (BN >= 128) return launch_gemm<BN, EPI_NORM_ROPE_BF16, kFp8>(tmA, tmB, tmD, p, st);
       break;
   }
   set_error("gemm: unknown epilogue %d", epi);
@@ -405,7 +533,7 @@ static int gemm_any(const void* A, const void* B, const float* scale_a, const fl
   if (fp8 && bn == 256) bn = 128;  // fp8 tiles hold a second (partial-sum) accumulator set: at most 128 columns
   G3C_REQUIRE(epilogue != EPI_NORM_ROPE_BF16 || bn >= 128, "gemm: the RMSNorm/RoPE epilogue needs tiles of whole heads");
 
-  CUtensorMap tmA, tmB;
+  CUtensorMap tmA, tmB, tmD;
   const int esize = fp8 ? 1 : 2, bk = fp8 ? kBlockK<true> : kBlockK<false>;
   const CUtensorMapDataType dt = fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   uint64_t dimsA[2] = {(uint64_t)K, (uint64_t)M}, strA[1] = {(uint64_t)lda * esize};
@@ -416,12 +544,23 @@ static int gemm_any(const void* A, const void* B, const float* scale_a, const fl
   uint32_t boxB[2] = {(uint32_t)bk, (uint32_t)bn};
   rc = make_tmap_bf16_sw128(&tmB, B, 2, dimsB, strB, boxB, dt);
   if (rc) return rc;
+  // D in boxes of 64 rows x 128 bytes (the epilogue's staging layout); TMA clips rows >= M and columns >= n_tma
+  const bool f32_out = epilogue == G3C_EPI_GATED_RESIDUAL_F32 || epilogue == G3C_EPI_F32;
+  const int dsize = f32_out ? 4 : 2;
+  const int n_tma = N / (16 / dsize) * (16 / dsize);
+  // with n_tma = 0 the map is never used (the dimension must not be empty)
+  uint64_t dimsD[2] = {(uint64_t)(n_tma > 0 ? n_tma : 16 / dsize), (uint64_t)M}, strD[1] = {(uint64_t)ldd * dsize};
+  uint32_t boxD[2] = {(uint32_t)(128 / dsize), (uint32_t)OUT_BOX_ROWS};
+  rc = make_tmap_bf16_sw128(&tmD, D, 2, dimsD, strD, boxD,
+                            f32_out ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
+  if (rc) return rc;
 
   GemmParams p;
   p.M = M;
   p.N = N;
   p.K = K;
   p.ldd = ldd;
+  p.n_tma = n_tma;
   p.D = D;
   p.gate = gate;
   p.nr_gamma = norm_rope ? norm_rope->gamma : nullptr;
@@ -438,12 +577,12 @@ static int gemm_any(const void* A, const void* B, const float* scale_a, const fl
   if (sn < 1) sn = 1;
   if (sn > p.num_n_blk) sn = p.num_n_blk;
   p.super_n = sn;
-  if (fp8) return bn == 64 ? dispatch_epi<64, true>(epilogue, tmA, tmB, p, st)
-                           : dispatch_epi<128, true>(epilogue, tmA, tmB, p, st);
+  if (fp8) return bn == 64 ? dispatch_epi<64, true>(epilogue, tmA, tmB, tmD, p, st)
+                           : dispatch_epi<128, true>(epilogue, tmA, tmB, tmD, p, st);
   switch (bn) {
-    case 64: return dispatch_epi<64, false>(epilogue, tmA, tmB, p, st);
-    case 128: return dispatch_epi<128, false>(epilogue, tmA, tmB, p, st);
-    default: return dispatch_epi<256, false>(epilogue, tmA, tmB, p, st);
+    case 64: return dispatch_epi<64, false>(epilogue, tmA, tmB, tmD, p, st);
+    case 128: return dispatch_epi<128, false>(epilogue, tmA, tmB, tmD, p, st);
+    default: return dispatch_epi<256, false>(epilogue, tmA, tmB, tmD, p, st);
   }
 }
 
