@@ -27,9 +27,10 @@ E4M3 = torch.float8_e4m3fn
 
 # The per-element constants below are set to about 4x the largest ratio observed over the cases of this file on one
 # H100 80GB HBM3 (132 SMs, 700 W power limit).
-# bf16 operands, fp32 wgmma sums: |error| / S reached 1.20e-6 (about 20 * 2^-24).  S grows with K as fast as the
-# error's worst case does, so the ratio does not grow like sqrt(K) * 2^-24 (7.6e-6 at K = 16384): it stays at a few
-# roundings of the tensor core's sum, whatever K.
+# bf16 operands, fp32 wgmma sums: |error| / S reached 1.20e-6 (about 20 * 2^-24).  S grows with K, and the ratio stays
+# at a few roundings of the tensor core's sum rather than growing like sqrt(K) * 2^-24 (7.6e-6 at K = 16384).  It is not
+# quite flat: at the engine's shapes (test_engine_shapes_gpu.py) it went from 2.8e-7 at K = 384 to 7.6e-7 at K = 4096
+# and 1.5e-6 at K = 16384, the largest K the engine runs.
 C32 = 4.5e-6
 # fp8 operands: 3.6e-4 (about 2^-11.5; 2.0e-4 over the shape matrix).  The e4m3 instruction keeps only about 14 bits of
 # its own k32 sum (the DeepSeek-V3 report measured the same on Hopper), so every element carries that much of its S.
