@@ -90,6 +90,8 @@ SIGNATURES = {
     "g3c_ln_modulate_fp8": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _F, _P]),
     "g3c_attn_fwd": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _F, _P]),
     "g3c_attn_fwd_sbhd": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _F, _P]),
+    "g3c_attn_fwd_sbhd_lse": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _F, _P]),
+    "g3c_attn_bwd_sbhd": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P] + [_I] * 12 + [_F, _P]),
     "g3c_attn_set_trace": (_I, [_P]),
     "g3c_ln_modulate": (_I, [_P, _P, _P, _P, _P, _I, _I, _F, _P]),
     "g3c_rmsnorm_rope": (_I, [_P, _I, _I, _I, _P, _P, _F, _P]),

@@ -6,7 +6,11 @@
 
 Supported: bf16 CUDA ``sbhd`` tensors, head_dim 128, any batch and any query / key count, no mask, no dropout, no bias,
 as many key heads as query heads, and context parallelism (K and V all-gathered over the group).  Anything else raises
-``NotImplementedError`` (unsupported configuration) or ``ValueError`` (malformed tensor); there is no fallback."""
+``NotImplementedError`` (unsupported configuration) or ``ValueError`` (malformed tensor); there is no fallback.
+
+Differentiable like TE's operator: gradients reach q, k and v through the native backward kernels
+(``ops.attention_sbhd``), and under context parallelism the K/V gather's backward reduce-scatters the gathered
+gradients over the group, so each rank receives the gradient of its own K/V slice."""
 from __future__ import annotations
 
 import math
@@ -15,6 +19,27 @@ from typing import Optional
 import torch
 
 from . import ops
+
+
+class _GatherSequence(torch.autograd.Function):
+    """all_gather_into_tensor over `group` along dim 0 (rank order); backward: reduce_scatter_tensor (sum) of the
+    gradient, so each rank gets the sum over ranks of the gradient of its own slice."""
+
+    @staticmethod
+    def forward(ctx, t, group):
+        ctx.group = group
+        world = torch.distributed.get_world_size(group)
+        out = torch.empty((world * t.shape[0],) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
+        torch.distributed.all_gather_into_tensor(out, t.contiguous(), group=group)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        world = torch.distributed.get_world_size(ctx.group)
+        out = torch.empty((grad.shape[0] // world,) + tuple(grad.shape[1:]), dtype=grad.dtype, device=grad.device)
+        torch.distributed.reduce_scatter_tensor(out, grad.contiguous(), op=torch.distributed.ReduceOp.SUM,
+                                                group=ctx.group)
+        return out, None
 
 
 class DotProductAttention(torch.nn.Module):
@@ -51,10 +76,7 @@ class DotProductAttention(torch.nn.Module):
         self.cp_group, self.cp_ranks, self.cp_stream = cp_group, cp_ranks, cp_stream
 
     def _gather(self, t: torch.Tensor) -> torch.Tensor:
-        world = torch.distributed.get_world_size(self.cp_group)
-        out = torch.empty((world * t.shape[0],) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
-        torch.distributed.all_gather_into_tensor(out, t.contiguous(), group=self.cp_group)
-        return out
+        return _GatherSequence.apply(t, self.cp_group)
 
     def forward(self, query_layer: torch.Tensor, key_layer: torch.Tensor, value_layer: torch.Tensor,
                 core_attention_bias_type: str = "no_bias",

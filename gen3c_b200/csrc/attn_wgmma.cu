@@ -10,6 +10,7 @@
 //                                             all-gather, 1 otherwise)
 //   O  [Lq, heads*128]
 //   kVTokenMajor (g3c_attn_fwd_sbhd): V [Lk, heads*128] token-major like K, any Lk >= 1, heads = batch x heads of sbhd
+//   kLse (g3c_attn_fwd_sbhd_lse, with kVTokenMajor): also lse [heads][Lq] f32 for the backward (attn_bwd_wgmma.cu)
 //
 // One CTA = ATT_ROWS_PER_CTA (128) query rows of one head, 384 threads (three warpgroups):
 //   warpgroup 0     TMA producer: Q once, then K_j and V^T_j through two rings of ATT_STAGES 32 KB stages each (a K
@@ -83,6 +84,7 @@ struct AttnParams {
   unsigned long long* wait_ns;         // optional profiling counter: ns spent polling chunk flags, summed over CTAs
   unsigned long long* trace;           // kTrace only: [3 roles][64 steps][8 slots] clock64 stamps of CTA (0,0), see
                                        // g3c_attn_set_trace in include/gen3c_b200.h
+  float* lse;                          // kLse only: [heads][Lq] log-sum-exp of each query row, log2 units of s sl2
 };
 
 static unsigned long long* g_attn_trace = nullptr;
@@ -94,12 +96,6 @@ static unsigned long long* g_attn_trace = nullptr;
         p.trace[((role) * 64 + j) * 8 + (slot)] = clock64();                                                \
     }                                                                                                       \
   } while (0)
-
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;\n" : "=f"(y) : "f"(x));
-  return y;
-}
 
 // S <- P = 2^(S sl2 - m) in place against the reference m of this thread's two rows; acc[h] += this thread's sum of
 // its 32 P of row h.
@@ -206,8 +202,10 @@ __device__ __forceinline__ void pack_p(uint32_t (&pa)[32], const float (&s)[64])
 }
 
 // kVTokenMajor: V is [Lk, heads*128] like K (instead of the chunked V^T), any Lk >= 1 (the last KV tile is partial and
-// masked), no context-parallel gate.
-template <bool kTrace, bool kVTokenMajor = false>
+// masked), no context-parallel gate.  kLse (with kVTokenMajor, for the backward of attn_bwd_wgmma.cu): also store
+// lse = m + log2(l) of each query row, from the final reference m and the quad-reduced l of the normalisation, so
+// 2^(s sl2 - lse) is the row's softmax whatever m the lazy rescale or the sum guard left.
+template <bool kTrace, bool kVTokenMajor = false, bool kLse = false>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
     k_attn_fwd(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
@@ -454,6 +452,10 @@ __global__ void __launch_bounds__(ATT_THREADS, 1)
       l += __shfl_xor_sync(0xffffffffu, l, 1);
       l += __shfl_xor_sync(0xffffffffu, l, 2);
       inv[h] = 1.0f / l;
+      if constexpr (kLse) {
+        const int row = q0 + (int)(c * 64 + warp * 16 + lane / 4) + 8 * h;
+        if (lane % 4 == 0 && row < p.Lq) p.lse[(size_t)head * p.Lq + row] = m_ref[h] + log2f(l);
+      }
     }
     const int row_a = q0 + (int)(c * 64 + warp * 16 + lane / 4);
 #pragma unroll
@@ -477,7 +479,7 @@ static int make_tmap_tokens(CUtensorMap* m, const void* base, int rows, int head
 }
 
 // scale = ln 2 declares that Q already carries softmax scale * log2(e): S is then in log2 units
-static float scale_log2(float scale) {
+float attn_scale_log2(float scale) {
   const float s = scale * 1.4426950408889634f;
   return fabsf(s - 1.0f) < 1e-6f ? 1.0f : s;
 }
@@ -520,7 +522,7 @@ int attn_fwd(const void* q, const void* k, const void* vt, void* o, int Lq, int 
   p.ldo = ldo;
   p.vt_chunk_len = vt_chunk_len;
   p.O = reinterpret_cast<__nv_bfloat16*>(o);
-  p.scale_log2 = scale_log2(scale);
+  p.scale_log2 = attn_scale_log2(scale);
   p.chunk_flags = gate ? gate->flags : nullptr;
   p.peer_timeout_ns = gate ? peer_timeout_ns() : G3C_MBAR_TIMEOUT_NS;
   p.wait_ns = gate ? gate->wait_ns : nullptr;
@@ -536,9 +538,10 @@ int attn_fwd(const void* q, const void* k, const void* vt, void* o, int Lq, int 
 }
 
 // q, k, v, o: `batch` x `heads` heads of 128 per token (the rows of contiguous sbhd [s, b, h, 128] tensors viewed as
-// [s, b*h*128]), so the batch is b*h heads of one launch.  V token-major like K; any Lq, Lk >= 1.
-int attn_fwd_sbhd(const void* q, const void* k, const void* v, void* o, int Lq, int Lk, int batch, int heads, int ldq,
-                  int ldk, int ldv, int ldo, float scale, cudaStream_t st) {
+// [s, b*h*128]), so the batch is b*h heads of one launch.  V token-major like K; any Lq, Lk >= 1.  lse (or NULL):
+// f32 [batch*heads][Lq], written by the kLse build of the same kernel.
+int attn_fwd_sbhd(const void* q, const void* k, const void* v, void* o, float* lse, int Lq, int Lk, int batch,
+                  int heads, int ldq, int ldk, int ldv, int ldo, float scale, cudaStream_t st) {
   G3C_REQUIRE(q && k && v && o, "attn_sbhd: null operand");
   G3C_REQUIRE(Lq > 0 && Lk > 0, "attn_sbhd: Lq=%d and Lk=%d must be >= 1", Lq, Lk);
   G3C_REQUIRE(batch > 0 && heads > 0 && (long long)batch * heads <= 65535,
@@ -551,6 +554,7 @@ int attn_fwd_sbhd(const void* q, const void* k, const void* v, void* o, int Lq, 
   G3C_REQUIRE(((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
                 reinterpret_cast<uintptr_t>(o)) & 15) == 0,
               "attn_sbhd: q, k, v and o must be 16-byte aligned");
+  G3C_REQUIRE((reinterpret_cast<uintptr_t>(lse) & 3) == 0, "attn_sbhd: lse must be 4-byte aligned");
   CUtensorMap tmQ, tmK, tmV;
   int rc = make_tmap_tokens(&tmQ, q, Lq, bh, ldq);
   if (rc) return rc;
@@ -561,6 +565,8 @@ int attn_fwd_sbhd(const void* q, const void* k, const void* v, void* o, int Lq, 
   static bool configured = false;
   if (!configured) {
     G3C_CUDA(cudaFuncSetAttribute(k_attn_fwd<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
+    G3C_CUDA(cudaFuncSetAttribute(k_attn_fwd<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  ATT_SMEM));
     configured = true;
   }
   AttnParams p = {};
@@ -570,10 +576,12 @@ int attn_fwd_sbhd(const void* q, const void* k, const void* v, void* o, int Lq, 
   p.ldo = ldo;
   p.vt_chunk_len = Lk;
   p.O = reinterpret_cast<__nv_bfloat16*>(o);
-  p.scale_log2 = scale_log2(scale);
+  p.scale_log2 = attn_scale_log2(scale);
   p.peer_timeout_ns = G3C_MBAR_TIMEOUT_NS;
+  p.lse = lse;
   dim3 grid((Lq + ATT_TILE - 1) / ATT_TILE, bh);
-  k_attn_fwd<false, true><<<grid, ATT_THREADS, ATT_SMEM, st>>>(tmQ, tmK, tmV, p);
+  if (lse) k_attn_fwd<false, true, true><<<grid, ATT_THREADS, ATT_SMEM, st>>>(tmQ, tmK, tmV, p);
+  else k_attn_fwd<false, true><<<grid, ATT_THREADS, ATT_SMEM, st>>>(tmQ, tmK, tmV, p);
   G3C_CUDA(cudaGetLastError());
   return G3C_OK;
 }
@@ -605,5 +613,16 @@ extern "C" int g3c_attn_fwd_gated(const void* q, const void* k, const void* vt, 
 
 extern "C" int g3c_attn_fwd_sbhd(const void* q, const void* k, const void* v, void* o, int Lq, int Lk, int batch,
                                  int heads, int ldq, int ldk, int ldv, int ldo, float scale, void* stream) {
-  return g3c::attn_fwd_sbhd(q, k, v, o, Lq, Lk, batch, heads, ldq, ldk, ldv, ldo, scale, (cudaStream_t)stream);
+  return g3c::attn_fwd_sbhd(q, k, v, o, nullptr, Lq, Lk, batch, heads, ldq, ldk, ldv, ldo, scale,
+                            (cudaStream_t)stream);
+}
+
+extern "C" int g3c_attn_fwd_sbhd_lse(const void* q, const void* k, const void* v, void* o, float* lse, int Lq, int Lk,
+                                     int batch, int heads, int ldq, int ldk, int ldv, int ldo, float scale,
+                                     void* stream) {
+  if (!lse) {
+    g3c::set_error("attn_sbhd_lse: null lse");
+    return G3C_EINVAL;
+  }
+  return g3c::attn_fwd_sbhd(q, k, v, o, lse, Lq, Lk, batch, heads, ldq, ldk, ldv, ldo, scale, (cudaStream_t)stream);
 }

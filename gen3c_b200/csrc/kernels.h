@@ -36,6 +36,9 @@ constexpr int ATT_ROWS_PER_CTA = 128;
 int attn_fwd(const void* q, const void* k, const void* vt, void* o, int Lq, int Lk, int heads,
              int ldq, int ldk, int ldo, int vt_chunk_len, float scale, cudaStream_t st,
              const ChunkGate* gate = nullptr);
+// log2-unit score scale of the attention kernels: fp32(scale * log2(e)), exactly 1 within 1e-6 of it (scale = ln 2
+// declares that Q already carries softmax scale * log2(e))
+float attn_scale_log2(float scale);
 
 struct PatchSrc {
   const __nv_bfloat16* ptr[4];

@@ -188,10 +188,8 @@ def _token_stride(t: torch.Tensor, name: str) -> int:
     return ld
 
 
-def attention_sbhd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Optional[float] = None) -> torch.Tensor:
-    """TE DotProductAttention(qkv_format="sbhd") semantics on the native kernel: q [sq, b, h, 128], k and v
-    [sk, b, h, 128] (V as given, any sq, sk >= 1) -> o [sq, b, h*128] = softmax(q k^T * scale) v per (batch, head).
-    scale defaults to 1/sqrt(128).  Unsupported shapes raise NotImplementedError, malformed tensors ValueError."""
+def _sbhd_operands(q, k, v):
+    """Checks of attention_sbhd; returns the token strides of q, k and v."""
     if q.dim() == 4 and q.shape[-1] != 128:
         raise NotImplementedError(f"head_dim {q.shape[-1]}: only 128 is implemented")
     if q.dim() == 4 and k.dim() == 4 and k.shape[2] != q.shape[2]:
@@ -202,15 +200,93 @@ def attention_sbhd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Opt
                          "and k, v in s")
     if not (q.device == k.device == v.device):
         raise ValueError("q, k and v must be on one device")
+    return ldq, ldk, ldv
+
+
+def _attention_sbhd_fwd(q, k, v, scale, with_lse):
+    """o [sq, b, h*128] of g3c_attn_fwd_sbhd, or (o, lse) of g3c_attn_fwd_sbhd_lse."""
+    ldq, ldk, ldv = _sbhd_operands(q, k, v)
     sq, b, h, d = q.shape
     o = torch.empty((sq, b, h * d), device=q.device, dtype=torch.bfloat16)
+    lse = torch.empty((b * h, sq), device=q.device, dtype=torch.float32) if with_lse else None
     if scale is None:
         scale = 128 ** -0.5
     lib = _lib.load()
     with torch.cuda.device(q.device):
-        _lib.check(lib.g3c_attn_fwd_sbhd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), sq, k.shape[0], b, h,
-                                         ldq, ldk, ldv, b * h * d, scale, _lib.stream_ptr()), "g3c_attn_fwd_sbhd")
+        args = (sq, k.shape[0], b, h, ldq, ldk, ldv, b * h * d, scale, _lib.stream_ptr())
+        if with_lse:
+            _lib.check(lib.g3c_attn_fwd_sbhd_lse(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(),
+                                                 *args), "g3c_attn_fwd_sbhd_lse")
+            return o, lse
+        _lib.check(lib.g3c_attn_fwd_sbhd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), *args),
+                   "g3c_attn_fwd_sbhd")
     return o
+
+
+def attention_sbhd_lse(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor,
+                       scale: Optional[float] = None) -> tuple[torch.Tensor, torch.Tensor]:
+    """attention_sbhd that also returns lse f32 [b*h, sq], each query row's log-sum-exp in log2 units of
+    q.k * scale * log2(e) (g3c_attn_fwd_sbhd_lse), for attention_sbhd_backward.  o equals attention_sbhd's bit for bit."""
+    return _attention_sbhd_fwd(q, k, v, scale, True)
+
+
+def attention_sbhd_backward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, o: torch.Tensor, lse: torch.Tensor,
+                            dout: torch.Tensor, scale: Optional[float] = None
+                            ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """(dq, dk, dv) of attention_sbhd_lse's (o, lse) for dout = dL/do (g3c_attn_bwd_sbhd): bf16, contiguous, in the
+    shapes of q, k and v.  o and dout [sq, b, h*128] (or [sq, b, h, 128]); bitwise reproducible."""
+    ldq, ldk, ldv = _sbhd_operands(q, k, v)
+    sq, b, h, d = q.shape
+    o4, do4 = o.view(sq, b, h, d), dout.reshape(sq, b, h, d)
+    ldo, lddo = _token_stride(o4, "o"), _token_stride(do4, "dout")
+    if lse.dtype != torch.float32 or tuple(lse.shape) != (b * h, sq) or not lse.is_contiguous():
+        raise ValueError(f"lse must be a contiguous float32 [{b * h}, {sq}] tensor")
+    if not (o.device == dout.device == lse.device == q.device):
+        raise ValueError("o, dout and lse must be on the device of q, k and v")
+    if scale is None:
+        scale = 128 ** -0.5
+    dq, dk, dv = (torch.empty(t.shape, device=q.device, dtype=torch.bfloat16) for t in (q, k, v))
+    delta = torch.empty((b * h, sq), device=q.device, dtype=torch.float32)
+    row = b * h * d
+    lib = _lib.load()
+    with torch.cuda.device(q.device):
+        _lib.check(lib.g3c_attn_bwd_sbhd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o4.data_ptr(), do4.data_ptr(),
+                                         lse.data_ptr(), delta.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
+                                         sq, k.shape[0], b, h, ldq, ldk, ldv, ldo, lddo, row, row, row, scale,
+                                         _lib.stream_ptr()), "g3c_attn_bwd_sbhd")
+    return dq, dk, dv
+
+
+class _AttentionSbhd(torch.autograd.Function):
+    """attention_sbhd inside an autograd graph: the LSE-saving forward, the native backward."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, scale):
+        o, lse = attention_sbhd_lse(q, k, v, scale)
+        ctx.save_for_backward(q, k, v, o, lse)
+        ctx.scale = scale
+        return o
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dout):
+        q, k, v, o, lse = ctx.saved_tensors
+        dq, dk, dv = attention_sbhd_backward(q, k, v, o, lse, dout.to(torch.bfloat16).contiguous(), ctx.scale)
+        return dq, dk, dv, None
+
+
+def attention_sbhd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Optional[float] = None) -> torch.Tensor:
+    """TE DotProductAttention(qkv_format="sbhd") semantics on the native kernel: q [sq, b, h, 128], k and v
+    [sk, b, h, 128] (V as given, any sq, sk >= 1) -> o [sq, b, h*128] = softmax(q k^T * scale) v per (batch, head).
+    scale defaults to 1/sqrt(128).  Unsupported shapes raise NotImplementedError, malformed tensors ValueError.
+    Differentiable: when grad mode is on and q, k or v requires grad, the forward also keeps each row's log-sum-exp and
+    the backward runs the native kernels of attention_sbhd_backward (bf16 gradients)."""
+    if scale is None:
+        scale = 128 ** -0.5
+    if torch.is_grad_enabled() and (q.requires_grad or k.requires_grad or v.requires_grad):
+        _sbhd_operands(q, k, v)
+        return _AttentionSbhd.apply(q, k, v, scale)
+    return _attention_sbhd_fwd(q, k, v, scale, False)
 
 
 def ln_modulate(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, pos: Optional[torch.Tensor] = None,

@@ -182,6 +182,27 @@ int g3c_attn_fwd(const void* q, const void* k, const void* vt, void* o, int Lq, 
 int g3c_attn_fwd_sbhd(const void* q, const void* k, const void* v, void* o, int Lq, int Lk, int batch, int heads,
                       int ldq, int ldk, int ldv, int ldo, float scale, void* stream);
 
+/* g3c_attn_fwd_sbhd that also stores, per (head, query row), the row's log-sum-exp for g3c_attn_bwd_sbhd:
+ *   lse f32 [batch*heads][Lq] (head-major, 4-byte aligned, non-NULL) = m + log2(l) in log2 units of s * sl2, where
+ *   s = q . k and sl2 = scale * log2(e) (exactly 1 for scale = ln 2), so softmax_j = 2^(s_j sl2 - lse).
+ *   O is bitwise equal to g3c_attn_fwd_sbhd's. */
+int g3c_attn_fwd_sbhd_lse(const void* q, const void* k, const void* v, void* o, float* lse, int Lq, int Lk, int batch,
+                          int heads, int ldq, int ldk, int ldv, int ldo, float scale, void* stream);
+
+/* Backward of g3c_attn_fwd_sbhd_lse: given dout = dL/dO, writes dq, dk, dv (bf16, the same sbhd token rows as q, k, v;
+ * leading dimensions lddq, lddk, lddv).  With P = 2^(s sl2 - lse) and Delta_i = sum_d dout_id o_id (fp32, from the
+ * bf16 o the forward returned):
+ *   dV = P^T dout,  dS = P o (dout V^T - Delta),  dQ = scale * dS K,  dK = scale * dS^T Q
+ * where scale is the natural-log softmax scale given to the forward (ln 2 under its log2 convention).  P and dS enter
+ * the MMAs as bf16, the products accumulate in fp32.  delta_ws is a caller-supplied f32 [batch*heads][Lq] workspace
+ * (overwritten with Delta); nothing is allocated.  Every gradient element has one writer (no atomics), so the result
+ * is bitwise reproducible.  Three launches on `stream`: Delta, then dK/dV (one CTA per 128 keys of a head), then dQ
+ * (one CTA per 128 queries of a head); S = q k^T and dout V^T are computed in both of the last two.  Sizes, strides
+ * and alignment as in g3c_attn_fwd_sbhd, for all ten tensors; lse and delta_ws 4-byte aligned. */
+int g3c_attn_bwd_sbhd(const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
+                      float* delta_ws, void* dq, void* dk, void* dv, int Lq, int Lk, int batch, int heads, int ldq,
+                      int ldk, int ldv, int ldo, int lddo, int lddq, int lddk, int lddv, float scale, void* stream);
+
 /* Profiling aid: when a device buffer of 3*64*8 uint64 is registered, the next g3c_attn_fwd launches run a
  * traced build of the kernel in which CTA (0,0) records clock64() stamps per KV step j (first 64 steps): roles 1/2 =
  * the two consumer warpgroups; slots 0 turn acquired, 1 MMAs of the step issued (S_j and P_{j-1} V_{j-1}), 2 S_j
